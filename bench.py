@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- decode tokens/sec of a LLaMA-7B-shaped model over the quantised KV cache (BASELINE.json's metric).
 
-    python bench.py --gpus N --steps K --warmup W [--workload NAME] [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--workload NAME] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one batch-1 decode step at cache length L of the named workload: for every layer q/k/v projection,
 fused device-side append (NUQ quantise + top-K outlier split + pack), fused attend over the packed cache
@@ -20,8 +20,12 @@ N > 1, one process per GPU under torch.distributed / NCCL, two layouts (--parall
 Both are strong scaling of the same fixed workload ("scaling": "strong").
 
 --impl reference: the reference's CPU implementation of the path, i.e. the C port of the kernel semantics
-(oracle/kvq_oracle_port.c; /root/reference does not exist on the GPU box and the reference's CPU path is Python)
-timed on the host cores over a bounded sample of the same workload.
+(oracle/kvq_oracle_port.c; the reference's own CPU path is Python) timed on the host cores over a bounded sample of
+the same workload.
+
+--dump-outputs DIR: after the timed steps, write the logits of the last timed step (what a caller of the decode step
+receives) to DIR/logits.npy as float32.  Weights, caches and token ids are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import json
@@ -37,18 +41,18 @@ sys.path.insert(0, ROOT)
 WORKLOADS = {
     # name: (model, bits, L (quantised slots), n_sink, outliers, description = BASELINE.json configs[i])
     #   outliers: "kv" = 1 % dense-and-sparse on K and V, "k" = capped K outliers only, "none" = dense-only
-    "7b-3b-128k": ("7b", 3, 131072, 5, "kv", "LLaMA-7B 3b NUQ + 1% outliers + 5 fp16 sink tokens, seqlen 128K, 1xB200 (configs[2])"),
+    "7b-3b-128k": ("7b", 3, 131072, 5, "kv", "LLaMA-7B 3b NUQ + 1% outliers + 5 fp16 sink tokens, seqlen 128K, 1xH100 (configs[2])"),
     "7b-4b-128k": ("7b", 4, 131072, 0, "kv", "LLaMA-7B 4b NUQ + 1% outliers, seqlen 128K (north_star roofline target)"),
-    "7b-4b-32k": ("7b", 4, 32768, 0, "kv", "LLaMA-7B 4b NUQ + 1% outliers, seqlen 32K, 1xB200 decode (configs[1])"),
+    "7b-4b-32k": ("7b", 4, 32768, 0, "kv", "LLaMA-7B 4b NUQ + 1% outliers, seqlen 32K, 1xH100 decode (configs[1])"),
     "7b-4b-4k": ("7b", 4, 4096, 0, "kv", "single-node smoke size"),
-    "7b-4b-1m": ("7b", 4, 1048576, 0, "none", "LLaMA-7B 4b NUQ, seqlen 1M, layer-pipeline across 4xB200 (configs[3])"),
-    "13b-3b-1m": ("13b", 3, 1048576, 0, "k", "LLaMA-13B 3b NUQ + capped-K outliers, seqlen 1M, layer-pipeline across 8xB200 (configs[4])"),
+    "7b-4b-1m": ("7b", 4, 1048576, 0, "none", "LLaMA-7B 4b NUQ, seqlen 1M, layer-pipeline across 4xH100 (configs[3])"),
+    "13b-3b-1m": ("13b", 3, 1048576, 0, "k", "LLaMA-13B 3b NUQ + capped-K outliers, seqlen 1M, layer-pipeline across 8xH100 (configs[4])"),
 }
 DEFAULT_WORKLOAD = "7b-3b-128k"   # BASELINE.json's metric is quoted at seqlen 128K; this config fits one GPU
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index=0):
         self.index, self.rows, self.proc = index, [], None
@@ -102,7 +106,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s), not a measured peak"
 
 
 def build_quantizer(cfg_bits, H, device):
@@ -222,7 +226,7 @@ def _time_cuda(fn, iters, warm=2):
 
 def reference_cuda_anchor(lc, cfg, L, n_sink, bits, ms_ours, peak):
     """The kernel-vs-kernel anchor (SURVEY 2.2 / 8d): the reference's OWN CUDA kernels (oracle/_ref/quant_cuda_ref.so =
-    deployment/kvquant/quant_cuda_kernel.cu compiled unmodified for sm_100a by oracle/build_ref.py) on this GPU, on one
+    deployment/kvquant/quant_cuda_kernel.cu compiled unmodified for sm_90a by oracle/build_ref.py) on this GPU, on one
     layer's cache of this workload: its K op (dense + SPMV_ATOMIC_ROPE_BALANCED) and V op (dense + SPMV_ATOMIC_BALANCED)
     -- the two launches of the chain modeling_llama.py:1963-1999, without its torch glue -- next to our fused attend."""
     import torch
@@ -251,7 +255,7 @@ def reference_cuda_anchor(lc, cfg, L, n_sink, bits, ms_ours, peak):
     chain = ms_k + ms_v
     return {"k_op_ms": ms_k, "v_op_ms": ms_v, "chain_ms": chain, "gbs": nbytes / chain / 1e6,
             "frac": nbytes / chain / 1e6 / peak, "ours_ms": ms_ours, "speedup": chain / ms_ours,
-            "what": "reference quant_cuda kernels (unmodified, sm_100a) on one layer of this workload, same GPU, same cache"}
+            "what": "reference quant_cuda kernels (unmodified, sm_90a) on one layer of this workload, same GPU, same cache"}
 
 
 def north_star_anchor(dev, cfg7b_like, peak, L=131072, n_caches=3):
@@ -287,20 +291,6 @@ def north_star_anchor(dev, cfg7b_like, peak, L=131072, n_caches=3):
     return rec
 
 
-def ncu_traffic(bits, L):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one fused attend (all its kernels), per launch, from the
-    committed ncu --set full capture of the same shape (profiles/ncu_traffic.json); None when no capture matches."""
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")
-    try:
-        with open(path) as f:
-            for e in json.load(f)["entries"]:
-                if e["bits"] == bits and abs(e["L"] - L) <= 1024:
-                    return e["dram_bytes_per_launch"]
-    except (OSError, KeyError, ValueError):
-        pass
-    return None
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -324,6 +314,8 @@ def main():
                          "theirs and merges (validated against NCCL at 2/4/8 GPUs, tests/test_zz_p2p_exchange.py); "
                          "nccl: all_gather + merge kernel")
     ap.add_argument("--torch-profile", default="", help="write a per-kernel table of 3 graph replays to this file (diagnostic)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the logits of the last timed step to DIR/logits.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -508,6 +500,7 @@ def main():
     if rank == 0:
         sampler.start()
     ms_total = timed(lambda i: step_device(), args.steps)
+    last_logits = logits_dev[0].float().cpu().numpy() if (args.dump_outputs and rank == 0) else None
     for i in range(args.warmup):
         step_e2e(i)
     ms_e2e = timed(step_e2e, args.steps)
@@ -573,7 +566,6 @@ def main():
             del mulK, pV
         ach = b_att / ms_att / 1e6
         roof = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": ncu_traffic(bits, Lq),
                 "peak_source": peak_src,
                 "kernel": "kvq_attend = attend_init + k_outlier_pers + k_scores(3) + v_native + attend_combine",
                 "algorithmic_bytes_per_launch": b_att, "ms_per_launch": ms_att,
@@ -593,6 +585,9 @@ def main():
                                                           cfg.n_layers, cfg.rope_theta, n_sink, repeats=5)
             cpu_b = {"value": tok_s, "unit": "tokens/s", "cores": cores, "kind": "port", "sample": sample}
 
+    if last_logits is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), last_logits)
     if rank == 0:
         setup = dict(cache_fill_s=round(t_fill, 1), weight_bytes=stage.weight_bytes(),
                      cache_bytes_per_layer=kd.layer_step_bytes(cfg, L), table_precision=stage.layers[0].cache.precision,

@@ -1,5 +1,5 @@
 /*
- * kvquant_b200 -- C ABI of the B200-native KVQuant deployment hot path.
+ * kvquant_b200 -- C ABI of the H100-native KVQuant deployment hot path.
  *
  * This header is the drop-in boundary (SURVEY.md section 8b).  Every entry point takes plain device pointers,
  * sizes and a CUDA stream; nothing here mentions torch.  The reference binds the same operations through
@@ -127,7 +127,7 @@ KVQ_API int kvq_v_matvec(int bits, const float* score, const int32_t* cache, flo
  *             (one 4-byte lookup per element), results equal to the legacy op chain to ~1e-6;
  *   non-NULL  fp16 mode (north_star: "fp16 LUT"): half2 table from kvq_rope_table_build_half (same theta, same
  *             rope_npos); the K tables (LUT*q_c, s_c*LUT*q_{c^64}) and cos/sin are fp16, every product is exact and
- *             every sum is fp32 (sm_100 mixed-precision FMA).  ~20 % faster K kernel; output within 1e-3 of the exact
+ *             every sum is fp32 (each fp16 product widened exactly to fp32).  ~20 % faster K kernel; output within 1e-3 of the exact
  *             result at a few thousand tokens, 1.4e-3 .. 2e-3 at 128K.
  * V keeps fp32 tables and weights in both modes.
  * ------------------------------------------------------------------------------------------------------------- */

@@ -1,4 +1,4 @@
-"""kvquant_b200 -- B200-native (sm_100a) implementation of the KVQuant deployment hot path.
+"""kvquant_b200 -- H100-native (sm_90a) implementation of the KVQuant deployment hot path.
 
 Layout
   csrc/            hand-written CUDA kernels + the C ABI (include/kvquant_b200.h)

@@ -1,4 +1,4 @@
-// kvquant_b200 -- shared device helpers (sm_100a only).
+// kvquant_b200 -- shared device helpers (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda.h>
@@ -7,8 +7,8 @@
 
 #ifndef __CUDA_ARCH__
 #else
-#if __CUDA_ARCH__ < 1000
-#error "kvquant_b200 is written for sm_100a (B200) only"
+#if __CUDA_ARCH__ != 900
+#error "kvquant_b200 is written for sm_90a (H100) only"
 #endif
 #endif
 
@@ -110,8 +110,7 @@ __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
   else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
-// L2 cache policies (sm_100a only accepts the .L2::evict_* qualifiers on 256-bit loads; narrower loads take a
-// createpolicy descriptor through .L2::cache_hint)
+// L2 cache policies: a createpolicy descriptor passed through .L2::cache_hint
 __device__ __forceinline__ uint64_t policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));

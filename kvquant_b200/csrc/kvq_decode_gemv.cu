@@ -1,8 +1,7 @@
 // kvquant_b200 -- batch-1 fp16 GEMV of the LLaMA decode harness (kvquant_b200/decode.py) with the element-wise
 // neighbours fused in.  NOT part of the reference's quant_cuda surface (the reference calls cuBLAS through
 // nn.Linear, modeling_llama.py:1811-1813, 2004); it exists because at batch 1 the 13.2 GB of fp16 weights are a
-// pure HBM stream and the library GEMV reached 4.4 TB/s of the 6.5 TB/s this pool's B200s copy at, with an RMSNorm /
-// SwiGLU / cast launch in front of every call.
+// pure HBM stream, and the library GEMV comes with an RMSNorm / SwiGLU / cast launch in front of every call.
 //
 //   y[r] = (residual ? residual[r] : 0) + sum_k W[r,k] * f(x)[k]              W fp16 [N,K] row-major, fp32 accumulate
 //   f = identity on an fp16 or f32 vector | RMSNorm(x, norm_w) (HF LlamaRMSNorm rounding) | silu(gate) * up

@@ -4,12 +4,11 @@
 //   VecQuant3MatMulKernelNUQPerChannelTransposedRopeMHABatchedFusedOpt   3692-4115
 //
 // Same arithmetic as k_scores_kernel<3> (kvq_kscore.cu): T[h][c][code] = (LUT q_c, s_c LUT q_c^64), one LDS.64 +
-// one FFMA2 per element.  What differs is how the 96-bit code streams are fed:
+// two FFMA per element.  What differs is how the 96-bit code streams are fed:
 //   * every packed word is loaded exactly ONCE: the four 24-bit windows of a 32-channel group are funnel-shifted out
 //     of the current and the carried word (the generic kernel loads both words of every window: 8 loads per 3
-//     words, +30 % DRAM reads measured, profiles/r01_ncu_final_kernels.csv);
-//   * G = 8 heads per CTA (64 KiB of tables) -> H/8 head groups x 37 token ranges = 148 CTAs (the generic kernel's
-//     G = 16 gave 128 CTAs x 4 tiles where 3.46 were needed);
+//     words);
+//   * G = 8 heads per CTA (64 KiB of tables) -> H/8 head groups x (SMs / groups) token ranges, one CTA per SM;
 //   * token ranges are cut at warp granularity and a warp whose 32 tokens lie past the range skips the tile, so the
 //     last tile of a range costs only its live warps.
 #include "kvq_kscore.cuh"
@@ -183,7 +182,7 @@ int k_scores3_dispatch(const KParams& p, cudaStream_t st) {
     attr_done = true;
   }
   const int n_groups = (p.H + C::G - 1) / C::G;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t max_splits = sms / n_groups > 0 ? sms / n_groups : 1;

@@ -15,13 +15,13 @@
 //     warp lookup, and G = 16 (4-bit) / 32 (3-, 2-bit) heads share one CTA, so a token's cos/sin are loaded once per
 //     16-32 heads instead of once per 8;
 //   * cos/sin come from a half2 copy of the rope table (same reference expressions, rounded once), held in
-//     registers for all 64 pairs of the thread's token; products are exact in fp32 and accumulate in fp32 with the
-//     mixed-precision FMA of sm_100 (fma.rn.f32.f16 -> FHFMA, one issue slot, half-select operands);
+//     registers for all 64 pairs of the thread's token; products are exact in fp32 and accumulate in fp32 (each
+//     half is widened to fp32, then one FFMA);
 //   * the packed codes reach shared memory by TMA (cp.async.bulk.tensor.2d boxes of [W rows x 64 tokens], four per
 //     head slab) through a 5-8 stage full/empty mbarrier ring filled by a producer warp: 64+ KiB in flight per SM
 //     without spending registers or issue slots on global loads; a warp = 16 tokens x 2 channel halves, warps drift
 //     apart by up to a ring.
-// Per element: 1 PRMT (3-bit: SHF+LOP3) + 1 LDS.32 + 2 FHFMA.
+// Per element: 1 PRMT (3-bit: SHF+LOP3) + 1 LDS.32 + 2 half->float conversions + 2 FFMA.
 #include "kvq_kscore.cuh"
 #include <cuda_fp16.h>
 
@@ -55,14 +55,13 @@ template <int BITS> struct KFCfg {
   static constexpr uint32_t kStage = (kKFWarps / kBoxWarps) * kBox;   // one slab = one head x 16 warp columns = 256 tokens
 };
 
-// acc += a.h{0,1} * b.h{0,1}: exact product, fp32 accumulation (SASS: FHFMA with .H0/.H1 operand selects)
+// acc += a.h{0,1} * b.h{0,1}: fp16 -> fp32 is exact and so is the product of two fp16 in fp32, so widening first and
+// one fp32 FMA round exactly as a mixed-precision fp16 x fp16 + fp32 FMA would (sm_90 has no such instruction)
 __device__ __forceinline__ void fhfma_lo(float& acc, uint32_t a, uint32_t b) {
-  asm("{ .reg .b16 al, ah, bl, bh; mov.b32 {al,ah}, %1; mov.b32 {bl,bh}, %2; fma.rn.f32.f16 %0, al, bl, %0; }"
-      : "+f"(acc) : "r"(a), "r"(b));
+  acc = __fmaf_rn(__low2float(*reinterpret_cast<const __half2*>(&a)), __low2float(*reinterpret_cast<const __half2*>(&b)), acc);
 }
 __device__ __forceinline__ void fhfma_hi(float& acc, uint32_t a, uint32_t b) {
-  asm("{ .reg .b16 al, ah, bl, bh; mov.b32 {al,ah}, %1; mov.b32 {bl,bh}, %2; fma.rn.f32.f16 %0, ah, bh, %0; }"
-      : "+f"(acc) : "r"(a), "r"(b));
+  acc = __fmaf_rn(__high2float(*reinterpret_cast<const __half2*>(&a)), __high2float(*reinterpret_cast<const __half2*>(&b)), acc);
 }
 template <int IMM> __device__ __forceinline__ uint32_t lds_u32i(uint32_t addr) {
   uint32_t v;
@@ -89,8 +88,7 @@ __device__ __forceinline__ uint32_t ld_keep_u32(const uint32_t* p, uint64_t pol)
 // One head, this lane's half of one token.  A warp covers 16 tokens x 2 halves: lane = half * 16 + token, half 0 owns
 // the even channels of the head, half 1 the odd ones (even- and odd-channel tables sit in disjoint banks, and both
 // halves read the same packed word -> a broadcast), so a thread keeps cos/sin of only 32 pairs in registers and the
-// compiler has room to keep many lookups in flight (the 64-pair form ran at half the issue rate on shared-memory
-// latency, profiles/r02_ncu_attend_4b_v1.csv).  The two halves meet in one shuffle per head.
+// compiler has room to keep many lookups in flight (the 64-pair form stalls on shared-memory latency).  The two halves meet in one shuffle per head.
 //   st   = shared address of this lane's token column in the slab (row r at st + r * kRow)
 //   base = shared address of the head's table (256-byte aligned)
 //   hs   = per-lane constants of its half (see KFHalf)

@@ -9,20 +9,20 @@
 // which is the reference's per-channel sum with the two channels that share a rotary pair (j, j+64) taken together.
 //
 // Why: the per-channel form (kvq_kscore.cu) costs one 8-byte shared-memory lookup per ELEMENT and the SM's
-// load/store data path (one 128-byte wavefront per clock) was 87 % busy (profiles/r01_ncu_final_kernels.csv).
+// load/store data path (one 128-byte wavefront per clock) is what bounds it.
 // Here one lookup serves a PAIR: the table is indexed by both codes,
 //   T[h][j][a | b << BITS] = (A q_j + B q_j64,  A q_j64 - B q_j)            256 (4-bit) / 64 (3-bit) entries,
-// so an element costs half a lookup, half an FFMA2 and ~1 address op.  The tables of all 64 pairs x 8 heads would
+// so an element costs half a lookup, one FFMA and ~1 address op.  The tables of all 64 pairs x 8 heads would
 // need 1 MiB (4-bit) / 256 KiB (3-bit), so a CTA walks its token range in P passes over PP pairs each (8 x 8 pairs /
 // 2 x 32 pairs), rebuilding the 128 KiB table between passes; the running sum travels through the score buffer
 // (the thread that owns column t writes it and reads it back in the next pass: no atomics, deterministic).
 //
-//   * thread = token, 512-token tiles, G = 8 heads per CTA, grid = (148 / 4 token ranges) x (H / 8 head groups);
+//   * thread = token, 512-token tiles, G = 8 heads per CTA, grid = (SMs / head groups token ranges) x (H / 8 head groups);
 //   * packed words are prefetched one tile ahead into a rotating register buffer (evict-first), the pass's rope
 //     values likewise; 3-bit words are loaded exactly once (the 24-bit windows are funnel-shifted out of a carried
 //     word) -- the per-channel kernel re-read straddled words;
 //   * per 8 pairs: 4 logic ops to interleave the two code streams into (a | b << BITS) units, then per pair
-//     SHF + LOP3 (mask | table base) + LDS.64 + FFMA2.
+//     SHF + LOP3 (mask | table base) + LDS.64 + 2 FFMA.
 #include "kvq_kscore.cuh"
 
 namespace kvq {
@@ -232,7 +232,7 @@ static int launch_k_pair(const KParams& p, cudaStream_t st) {
   }
   const int n_groups = (p.H + C::G - 1) / C::G;
   const int64_t n_tiles = (p.L + C::TT - 1) / C::TT;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t max_splits = sms / n_groups > 0 ? sms / n_groups : 1;

@@ -17,7 +17,7 @@
 //   * thread = token (coalesced 128-byte warp loads straight from the sequence-fastest cache rows), per-channel
 //     premultiplied tables T[h][c][code] = (LUT*q[h,c], s_c*LUT*q[h,c^64]) in shared memory: 16 (8, 4) entries per
 //     channel are 16 distinct consecutive 8-byte slots -> conflict-free multicast for any code pattern.
-//   * per element: 1 address op (PRMT), 1 LDS.64, 1 packed FFMA2; words and rope values are prefetched into rotating
+//   * per element: 1 address op (PRMT), 1 LDS.64, 2 FFMA; words and rope values are prefetched into rotating
 //     register buffers; token ranges are cut at warp granularity so that every SM gets an equal share.
 #include "kvq_kscore.cuh"
 #include <cuda_fp16.h>
@@ -248,14 +248,14 @@ __global__ void __launch_bounds__(KCfg<BITS>::kThreads, 1) k_scores_kernel(const
 
 // ------------------------------------------------------------------------------------------------------------
 // kappa form of the dense kernel (alternative, KVQ_K_IMPL=kappa).  The LDS.64 form above pays two shared-memory wavefronts per 32
-// elements; profiling (profiles/r01_*) showed the shared-memory pipe 68 % busy and `mio_throttle` the top stall.
+// elements, and the shared-memory pipe is what limits it.
 // Here the shared table holds the RAW per-channel LUT (4 bytes per entry -> one wavefront per 32 elements) and the
 // query-dependent factor is applied arithmetically per (head, pair, token):
 //
-//     kappa = cos*(q_c, q_c64) + sin*(q_c64, -q_c)            2 packed ops, q pairs are uniform operands from the
-//     acc  += (LUT_c[code_c], LUT_c64[code_c64]) * kappa      constant bank (LDCU.128 -> FMUL2 / FFMA2 UR operands)
+//     kappa = cos*(q_c, q_c64) + sin*(q_c64, -q_c)            4 scalar ops, q pairs are uniform operands from the
+//     acc  += (LUT_c[code_c], LUT_c64[code_c64]) * kappa      constant bank (LDC.128 -> FMUL / FFMA UR operands)
 //
-// per pair: 2 PRMT + 2 LDS.32 + LDCU.128 + FMUL2 + 2 FFMA2  = 4 issue slots and 1 shared wavefront per element.
+// per pair: 2 PRMT + 2 LDS.32 + LDC.128 + 2 FMUL + 4 FFMA  = 8 issue slots and 1 shared wavefront per element.
 // The rotated-query constants live in __constant__ memory, refreshed per call by a tiny prep kernel + a D2D
 // cudaMemcpyToSymbolAsync (stream-ordered, graph-capturable).  K launches of one device must be stream-ordered.
 // ------------------------------------------------------------------------------------------------------------
@@ -280,10 +280,7 @@ __device__ __forceinline__ float lds_f1(uint32_t addr) {
   return v;
 }
 __device__ __forceinline__ float2 fmul2(const float2 a, const float2 b) {
-  float2 d;
-  asm("{ .reg .b64 ra, rb, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mul.rn.f32x2 rd, ra, rb; mov.b64 {%0,%1}, rd; }"
-      : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 }
 
 // one work item (head h (global), chunk a): 8 pairs
@@ -488,7 +485,7 @@ static int launch_k_kappa(const KParams& p, cudaStream_t st) {
   if (rc != 0) return rc;
   const int n_groups = (p.H + C::G - 1) / C::G;
   const int64_t n_tiles = (p.L + C::TT - 1) / C::TT;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t max_splits = sms / n_groups > 0 ? sms / n_groups : 1;
@@ -551,13 +548,12 @@ __global__ void __launch_bounds__(kOutThreads) k_outlier_kernel(
 // 8-byte rope read plus TWO scattered reads of q.  Here CTAs are persistent and keep (q[c], q[c^64]) for all channels
 // in shared memory (one 8-byte shared read per entry instead of two scattered global ones); the rope values still
 // come from the table.  In the fused path the sums go to a TOKEN-major partial buffer (a token's heads share one
-// 128-byte line, so a warp's ~25 reductions coalesce into one or two L1 requests: 46 -> 38 us at 128K).
-// Measured alternatives (DESIGN.md section 4.1): a second, token-major copy of the rope table read with coalesced
-// row loads + shuffles instead of the gather (59 us: it loads rows for the zero-valued pads too and adds 8 shuffles
-// per entry); evaluating cosf/sinf(theta_j * pos) per entry
-// instead of the gather (50 us vs 55 us at 128K, 40 M instead of 26 M warp instructions), and accumulating into a
-// per-CTA [H][256-token] shared tile with coalesced write-out instead of global atomics (85-98 us: shared-memory
-// fp32 atomics are compare-and-swap loops).
+// 128-byte line, so a warp's ~25 reductions coalesce into one or two L1 requests).
+// Alternatives considered (DESIGN.md section 4.1): a second, token-major copy of the rope table read with coalesced
+// row loads + shuffles instead of the gather (it loads rows for the zero-valued pads too and adds 8 shuffles per
+// entry); evaluating cosf/sinf(theta_j * pos) per entry instead of the gather (more instructions; used beyond
+// L2-sized rope tables, k_out_direct); accumulating into a per-CTA [H][256-token] shared tile with coalesced write-out
+// instead of global atomics (shared-memory fp32 atomics are compare-and-swap loops).
 constexpr int kOutPersThreads = 512;
 __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
     const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
@@ -632,10 +628,10 @@ static int k_out_impl_table() {   // KVQ_KOUT_IMPL=table selects the non-persist
 }
 
 // rope tables beyond this many positions are not gathered from by the outlier scatter (KVQ_KOUT_DIRECT_NPOS overrides):
-// 64 pairs x 8 bytes x 160K positions = 80 MB, about what stays resident in the 126 MB L2 next to the streams
+// 64 pairs x 8 bytes x 64K positions = 32 MB, about what stays resident in the 50 MB L2 next to the streams
 static bool k_out_direct(int64_t n_positions) {
   static int64_t thr = -1;
-  if (thr < 0) { const char* e = getenv("KVQ_KOUT_DIRECT_NPOS"); thr = e ? atoll(e) : 160 * 1024; }
+  if (thr < 0) { const char* e = getenv("KVQ_KOUT_DIRECT_NPOS"); thr = e ? atoll(e) : 64 * 1024; }
   return n_positions > thr;
 }
 
@@ -667,7 +663,7 @@ static int launch_k_outliers(const KParams& p, int zero_first, float scale, cuda
     if (e != cudaSuccess) return (int)e;
     smem_set = smem;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t want = (total + kOutPersThreads - 1) / kOutPersThreads;
@@ -713,7 +709,7 @@ static int launch_k_scores(const KParams& p, cudaStream_t st) {
     attr_done = true;
   }
   const int n_groups = (p.H + C::G - 1) / C::G;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t max_splits = sms / n_groups > 0 ? sms / n_groups : 1;
@@ -791,10 +787,8 @@ int k_scores_fused_fast(int bits, const float* q, const int32_t* cache, float* s
                         int pos_offset, float* gmax, float scale, const int64_t* len_dev, int64_t len_add, void* qtab,
                         cudaStream_t st) {
   // KVQ_K_BLOCK=<tokens>: walk the cache in blocks whose score rows (H x block floats) stay L2-resident between the
-  // outlier scatter (atomic adds) and the dense kernel.  Measured at 1M tokens, 3-bit, 1 % outliers with 128K blocks:
-  // outlier scatter 8 x 0.090 ms (one pass: 0.79 ms by table gather, 0.68 ms with direct cos/sin), dense kernel
-  // 8 x 0.156 ms (one pass: 1.17 ms), attend 3.13 ms vs 2.96 ms -- no gain, so the default is ONE pass; the switch
-  // stays for A/B runs and is covered by tests/test_gpu_variants.py.
+  // outlier scatter (atomic adds) and the dense kernel.  The default is ONE pass; the switch stays for A/B runs and is
+  // covered by tests/test_gpu_variants.py.
   static int64_t kBlock = 0;
   if (kBlock == 0) {
     const char* e = getenv("KVQ_K_BLOCK");

@@ -40,11 +40,10 @@ __device__ __forceinline__ float2 lds_f2(uint32_t addr) {
   asm("ld.shared.v2.f32 {%0,%1}, [%2+%3];" : "=f"(v.x), "=f"(v.y) : "r"(addr), "n"(IMM));
   return v;
 }
-// packed fp32 FMA (sm_100 FFMA2): acc.xy += a.xy * b.xy in one issue slot
+// acc.xy += a.xy * b.xy, each lane one fused, round-to-nearest fp32 FMA (sm_90 has no packed FFMA2: two FFMA)
 __device__ __forceinline__ void ffma2(float2& acc, const float2 a, const float2 b) {
-  asm("{ .reg .b64 ra, rb, rc; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mov.b64 rc, {%0,%1};"
-      " fma.rn.f32x2 rc, ra, rb, rc; mov.b64 {%0,%1}, rc; }"
-      : "+f"(acc.x), "+f"(acc.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
+  acc.x = __fmaf_rn(a.x, b.x, acc.x);
+  acc.y = __fmaf_rn(a.y, b.y, acc.y);
 }
 // effective length / per-CTA range of a launch whose length lives on the device (CUDA-graph replays with a growing
 // cache): the grid was sized for the cap p.L, the kernel re-derives its split from the current length

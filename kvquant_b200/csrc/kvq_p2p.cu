@@ -1,11 +1,11 @@
 // kvquant_b200 -- sequence-sharded decode: exchange of the per-GPU partial attention results over NVLink peer memory,
-// fused with their merge.  Validated on 2, 4 and 8 B200s against NCCL all_gather + kvq_attend_merge (bit-identical over
-// 200 rounds, tests/test_zz_p2p_exchange.py); measured at N = 2, 32K tokens: 165.8 vs 161.4 tokens/s.  It is the default
+// fused with their merge.  Validated against NCCL all_gather + kvq_attend_merge (bit-identical over
+// 200 rounds, tests/test_zz_p2p_exchange.py).  It is the default
 // of the sequence-sharded decode (bench.py --sp-exchange p2p).
 //
 // No counterpart in the reference (it never shards a layer's cache).  What it replaces here is
 //     dist.all_gather_into_tensor(parts) ; kvq_attend_merge(parts)            (kvquant_b200/decode.py)
-// i.e. a collective launch (~10-15 us of latency for 16.6 KB per rank) in front of a 2 us kernel, 32 times per token.
+// i.e. a collective launch in front of a tiny merge kernel, once per layer and token.
 //
 // Every rank owns one buffer, allocated with cudaMalloc and opened by its peers through CUDA IPC:
 //     float  data [2][world][H*129]     slot [b][r] = rank r's (out[H][128], lse[H]) of an exchange with parity b

@@ -461,7 +461,7 @@ int num_sms_cached() {
   int& n = g_sms[dev & 63];
   if (!n) {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }

@@ -9,7 +9,7 @@
 // The second term is one scalar per head.  The first needs only the global table, which lets TWO codes be looked up
 // at once: a byte (4-bit), a 6-bit field (3-bit) or a nibble (2-bit) of the packed word indexes a lane-private
 // table of float2 {cent[lo], cent[hi]} (lane-private = bank-conflict-free for any code pattern), and one packed
-// FFMA2 accumulates both channels:   1 address op + 1 LDS.64 + 1 FFMA2  per TWO elements.
+// lookup feeds both channels:   1 address op + 1 LDS.64 + 2 FFMA  per TWO elements.
 // What bounds this kernel is the SM's load/store data path (one 8-byte lookup per 2 elements plus the outlier
 // reductions), see DESIGN.md sections 4.2 and 7.
 //
@@ -22,11 +22,11 @@ namespace kvq {
 
 constexpr int kNThreads = 512;
 constexpr int kNT = 32;          // tokens per stage (128-byte rows, 128B swizzle)
-constexpr int kNMaxStages = 3;   // a 4th stage fits at 3 bits but measured no faster (0.395 vs 0.392 ms attend at 128K)
+constexpr int kNMaxStages = 3;   // a 4th stage fits at 3 bits
 constexpr int kNTokPerWarp = kNT / (kNThreads / 32);   // outlier rows handled by one warp per tile (2)
 // row strides of the staged weights (floats).  Lanes of a warp sit in up to 8 different heads (3-bit) and read the SAME
 // token columns: with 32-float rows every head's row starts in bank 0 -- an 8-way conflict on the LDS.128 of w*sf and a
-// ~25-way one on the outlier weight gather (ncu round 2: 6.3 M of 28.9 M shared wavefronts were conflicts at 3 bits).
+// ~25-way one on the outlier weight gather.
 constexpr int kNWStride = 33;    // w      : scalar gathers, head h token t -> bank (h + t) % 32
 constexpr int kNWsStride = 36;   // w * sf : 16-byte reads, head h chunk q -> bank group (h + q) % 8
 
@@ -75,9 +75,8 @@ __device__ __forceinline__ void red_add_f32(float* addr, float v) {
   asm volatile("red.relaxed.gpu.global.add.f32 [%0], %1;" ::"l"(addr), "f"(v) : "memory");
 }
 __device__ __forceinline__ void ffma2v(float2& acc, const float2 a, const float2 b) {
-  asm("{ .reg .b64 ra, rb, rc; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mov.b64 rc, {%0,%1};"
-      " fma.rn.f32x2 rc, ra, rb, rc; mov.b64 {%0,%1}, rc; }"
-      : "+f"(acc.x), "+f"(acc.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
+  acc.x = __fmaf_rn(a.x, b.x, acc.x);
+  acc.y = __fmaf_rn(a.y, b.y, acc.y);
 }
 
 // 32 tokens of one unit.  row_off/swz: this unit's word row in the 128B-swizzled stage; tab = shared address of the

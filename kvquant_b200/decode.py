@@ -284,7 +284,7 @@ class GraphedStage:
         The hop of the [hidden] fp16 vector is PART of the captured step: rank r's graph is
         `recv from r-1 -> its layers -> send to (r+1) % world`, rank 0 additionally owns a second graph
         `recv from world-1 -> norm + lm_head`.  NCCL send/recv kernels inside the graph cost microseconds per hop; issued
-        from the host (round 1) every hop paid ~0.8 ms of launch latency and the pipeline ran slower than one GPU."""
+        from the host every hop pays the launch latency of a host-issued collective."""
         self.stage = stage
         self.pp = pp
         dev = stage.device

@@ -14,7 +14,7 @@ def build(force=False):
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     if not force and os.path.exists(OUT) and os.path.getmtime(OUT) >= os.path.getmtime(SRC):
         return OUT
-    # -march=x86-64-v3 (AVX2/FMA): the .so is built in the CPU container and runs on the GPU box's host cores
+    # -march=x86-64-v3 (AVX2/FMA): the .so may be built on one x86-64 host and run on another (the GPU host's cores)
     cmd = ["gcc", "-O3", "-fopenmp", "-march=x86-64-v3", "-fPIC", "-shared", "-std=c11", SRC, "-o", OUT, "-lm"]
     subprocess.check_call(cmd)
     return OUT

@@ -2,7 +2,7 @@
 (quant/kvquant/simquant_module_quantizer.py: SimQuant.add_batch + SimQuant.quantize, the functions
 quant/llama_simquant.py:275 calls to fill quantizers.pickle) on small synthetic activations, on the CPU.
 
-    python tests/golden/gen_quantizers_golden.py        # needs /root/reference (this container only)
+    python tests/golden/gen_quantizers_golden.py        # needs a reference checkout (oracle/build_ref.py: REF_ROOT)
 
 The fixtures hold plain numpy arrays / floats in the reference's tuple layout, so the tests need neither torch
 pickles nor the reference at run time.
@@ -18,7 +18,9 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference/quant")
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "oracle"))
+from build_ref import REF_ROOT  # noqa: E402
+sys.path.insert(0, os.path.join(REF_ROOT, "quant"))
 from kvquant.simquant_module_quantizer import SimQuant  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Generate tests/golden/simquant_*.npz by importing the REFERENCE's own simulated-quant functions
-(/root/reference/quant/kvquant/simquant_module_quantizer.py: get_outliers, get_outliers_dynamic,
-quant_fn_nuq_recon, round_to_nearest_pole_sim) on CPU.  Run in the build container only
-(/root/reference does not exist on the GPU box); the produced fixtures are committed.
+(the reference's quant/kvquant/simquant_module_quantizer.py: get_outliers, get_outliers_dynamic,
+quant_fn_nuq_recon, round_to_nearest_pole_sim) on CPU.  Needs a reference checkout
+(oracle/build_ref.py: REF_ROOT); the produced fixtures are committed.
 
     python tests/golden/gen_simquant_golden.py
 """
@@ -15,7 +15,9 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference/quant")
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "oracle"))
+from build_ref import REF_ROOT  # noqa: E402
+sys.path.insert(0, os.path.join(REF_ROOT, "quant"))
 
 from kvquant.simquant_module_quantizer import (  # noqa: E402  (reference code, imported not copied)
     get_outliers, get_outliers_dynamic, quant_fn_nuq_recon, round_to_nearest_pole_sim)

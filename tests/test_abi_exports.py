@@ -1,4 +1,4 @@
-"""CPU: the C-ABI shared library builds (nvcc cross-compiles sm_100a without a GPU), loads, and exports every
+"""CPU: the C-ABI shared library builds (nvcc cross-compiles sm_90a without a GPU), loads, and exports every
 symbol include/kvquant_b200.h declares; the Python surface has exactly the reference's 34 operator names."""
 import ctypes
 import os

@@ -46,23 +46,69 @@ def test_host_generated_layer_has_the_cache_layout():
     assert 1 <= n <= len(os.sched_getaffinity(0)) and "affinity" in desc
 
 
-def test_reference_class_extraction_is_verbatim():
+SYNTH_MODELING = '''import math
+import torch
+import quant_cuda
+
+
+def helper():
+    return 1
+
+
+def compute_lut(x):   # trailing comment
+    return x * 2
+
+
+@torch.no_grad()
+class QuantK:
+    """keys"""
+    def f(self):
+        return quant_cuda.ping()
+
+
+X = 3
+
+
+class QuantV(object):
+
+    def g(self):   # blank line above kept
+        return compute_lut(3)
+
+
+class Other:
+    pass
+'''
+
+
+def test_reference_class_extraction_is_verbatim(tmp_path, monkeypatch):
+    """The cutter of oracle/build_ref_py.py on a stand-in for the reference's modeling file: the three definitions
+    (decorators included) land byte for byte behind the generated header, nothing else does."""
     import build_ref_py
-    if not os.path.exists(build_ref_py.SRC):
-        pytest.skip("/root/reference not present")
-    assert build_ref_py.build()
+    src = tmp_path / "modeling_llama.py"
+    src.write_text(SYNTH_MODELING)
+    real_out = build_ref_py.OUT
+    monkeypatch.setattr(build_ref_py, "SRC", str(src))
+    monkeypatch.setattr(build_ref_py, "OUT_DIR", str(tmp_path / "_ref"))
+    monkeypatch.setattr(build_ref_py, "OUT", str(tmp_path / "_ref" / "ref_cache_managers.py"))
+    assert build_ref_py.build(force=True)
     out = open(build_ref_py.OUT).read()
     tree = ast.parse(out)
     names = [n.name for n in tree.body if isinstance(n, (ast.FunctionDef, ast.ClassDef))]
     assert names == ["compute_lut", "QuantK", "QuantV"]
-    src = open(build_ref_py.SRC).read().splitlines(keepends=True)
-    ref_tree = ast.parse("".join(src))
-    for node in ref_tree.body:
+    lines = SYNTH_MODELING.splitlines(keepends=True)
+    for node in ast.parse(SYNTH_MODELING).body:
         if isinstance(node, (ast.FunctionDef, ast.ClassDef)) and node.name in build_ref_py.WANTED:
-            assert "".join(src[node.lineno - 1:node.end_lineno]) in out      # byte for byte
-    # the generated file lives in the git-ignored oracle/_ref/ only
-    assert os.path.dirname(build_ref_py.OUT).endswith(os.path.join("oracle", "_ref"))
-    rc = subprocess.run(["git", "check-ignore", "-q", build_ref_py.OUT], cwd=ROOT).returncode
+            first = min([node.lineno] + [d.lineno for d in node.decorator_list])
+            assert "".join(lines[first - 1:node.end_lineno]) in out      # byte for byte
+    assert "def helper" not in out and "class Other" not in out and "X = 3" not in out
+    # the loader binds `import quant_cuda` to the module it is given
+    fake = type(sys)("fake_quant_cuda")
+    fake.ping = lambda: "pong"
+    mod = build_ref_py.load(fake, "ref_managers_fake")
+    assert mod.quant_cuda is fake and mod.QuantK().f() == "pong" and mod.QuantV().g() == 6
+    # the real generated file lives in the git-ignored oracle/_ref/ only
+    assert os.path.dirname(real_out).endswith(os.path.join("oracle", "_ref"))
+    rc = subprocess.run(["git", "check-ignore", "-q", real_out], cwd=ROOT).returncode
     assert rc in (0, 128), "oracle/_ref/ref_cache_managers.py must stay out of history"   # 128: not a git checkout
 
 
