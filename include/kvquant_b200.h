@@ -153,7 +153,8 @@ KVQ_API int kvq_attend_merge(const float* parts, int n_parts, int H, float* out,
  *   kvq_append_kv_fused_dyn : writes slot  *len_dev + slot_add  (a full cache drops the token)
  *   kvq_attend_dyn          : attends over L = min(*len_dev + len_add, L_cap) slots; grids, scratch
  *                             (kvq_attend_scratch_bytes(H, L_cap)) and the rope table are sized for L_cap.
- *                             Native V form only (v_cent + v_aff); KVQ_E_UNSUPPORTED where kvq_attend would fall back.
+ *                             Native V form only (v_cent + v_aff); accepts every shape kvq_attend accepts (bits 2-4,
+ *                             H <= 64, H % 4 == 0).
  * ------------------------------------------------------------------------------------------------------------- */
 KVQ_API int kvq_append_kv_fused_dyn(int bits, int H, int64_t Lmax, const int64_t* len_dev, int64_t slot_add, int n_each,
                             const float* k_new, int32_t* kcache, const float* klut, const float* klut_sub,

@@ -7,8 +7,8 @@
 //
 //   O[h,c] = sum_t w[h,t] * (LUT[t, code(h,c,t)] (+) outlier(h,c,t))
 //
-// This file: the generic per-token-LUT kernel (legacy op surface, and the fused path's fallback for shapes whose native
-// tile does not fit shared memory), the attend_init / attend_combine / attend_merge kernels, the TMA descriptor helper
+// This file: the generic per-token-LUT kernel (legacy op surface, and the fused path over a cache given as
+// materialised LUT rows only), the attend_init / attend_combine / attend_merge kernels, the TMA descriptor helper
 // and the kvq_attend entry points.  The native fused-path V kernel is kvq_vnative.cu.
 //
 // Design (DESIGN.md section 4.2):
@@ -625,12 +625,10 @@ static int attend_impl(int bits, const float* q, const int32_t* kcache, const fl
       rc = k_scores_fused_fast(bits, q, kcache, scores, stride, klut, k_outliers, k_outlier_idx, n_out, H, Lmax, L,
                                rope_cos_sin, rope_half, rope_npos, theta, pos_offset, gmax, scale, len_dev, len_add, qtab, st);
     if (rc) return rc;
-    rc = KVQ_E_UNSUPPORTED;
-    if (native_v)
+    if (native_v) {
       rc = v_native_dispatch(bits, scores, stride, gmax, vcache, v_cent, v_aff, v_outliers, v_outlier_idx, n_out, H,
                              Lmax, L, part_o, part_l, &n_cta, len_dev, len_add, st);
-    // shapes whose native tile does not fit shared memory (e.g. 13B at 4 bits) fall back to the per-token-LUT kernel
-    if (rc == KVQ_E_UNSUPPORTED && vlut_tok != nullptr && len_dev == nullptr) {
+    } else {   // materialised per-token LUT rows (kvq_attend without v_cent / v_aff)
       VParams p{};
       p.score = scores; p.lut_tok = vlut_tok; p.out = part_o; p.out_l = part_l; p.gmax = gmax;
       p.outliers = v_outliers; p.outlier_idx = v_outlier_idx;

@@ -15,6 +15,10 @@
 //
 // Data movement: TMA (cp.async.bulk.tensor.2d, 128B swizzle, boxes of up to 256 rows) streams the
 // [H*W rows x 32 tokens] code slab of a tile into a 2-3 stage ring behind mbarriers; thread = packed word row.
+//
+// Head split: where the whole slab does not fit shared memory next to the table (4-bit at H >= 36, 3-bit at H >= 60),
+// the grid gains a second dimension of G = 2 head groups and CTA (r, g) streams only heads [g*H/2, (g+1)*H/2) of token
+// range r.  The two CTAs of a range write disjoint heads of the same partial row, so the combine is unchanged.
 #include "kvq_common.cuh"
 #include <stdlib.h>
 
@@ -124,17 +128,20 @@ __device__ __forceinline__ void vn_tile_unit(const unsigned char* stage, uint32_
   }
 }
 
-template <int BITS>
+// SPLIT: gridDim.y head groups (see the head split above); SPLIT = false is the whole-slab launch with h0 = 0
+template <int BITS, bool SPLIT>
 __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_constant__ CUtensorMap tmap, const VNParams p) {
   using C = VNCfg<BITS>;
   constexpr int N = C::N, W = C::W, NP = C::NP, TABN = C::TABN;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int rows = p.H * W;
-  const VNSmem lay = vn_smem_layout(rows, TABN, p.H, p.n_stages);
+  const int Hg = SPLIT ? p.H / (int)gridDim.y : p.H;     // heads of this CTA: [h0, h0 + Hg)
+  const int h0 = SPLIT ? (int)blockIdx.y * Hg : 0;
+  const int rows = Hg * W;
+  const VNSmem lay = vn_smem_layout(rows, TABN, Hg, p.n_stages);
   float2* s_tab = reinterpret_cast<float2*>(smem + lay.off_tab);   // [TABN][32 lanes]
-  float* s_w = reinterpret_cast<float*>(smem + lay.off_w);         // [2][H][kNWStride]    w = exp(s - max)
-  float* s_ws = reinterpret_cast<float*>(smem + lay.off_ws);       // [2][H][kNWsStride]   w * sf_t
+  float* s_w = reinterpret_cast<float*>(smem + lay.off_w);         // [2][Hg][kNWStride]    w = exp(s - max)
+  float* s_ws = reinterpret_cast<float*>(smem + lay.off_ws);       // [2][Hg][kNWsStride]   w * sf_t
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem + lay.off_bar);
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -148,14 +155,14 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
   }
   const uint32_t tab = smem_u32(s_tab) + lane * 8;
 
-  // ---- thread -> unit mapping (same as kvq_vaccum.cu) ------------------------------------------------------------
+  // ---- thread -> unit mapping (same as kvq_vaccum.cu); u_head is relative to h0 -------------------------------------
   int u_row[2], u_head[2], u_ch0[2], u_part[2];
   bool u_on[2];
   int sub = 0;
   if constexpr (BITS == 3) {
     sub = warp % 3;
     const int tri = warp / 3;
-    const int ngroups = p.H * 4;
+    const int ngroups = Hg * 4;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int gi = tri * 32 + lane + i * 160;
@@ -166,7 +173,7 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
       u_part[i] = 0;
     }
   } else {
-    const int nunits = p.H * 16;
+    const int nunits = Hg * 16;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int u = tid + i * kNThreads;
@@ -194,10 +201,10 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
     for (int k = 0; k < NP; ++k) acc[i][k] = make_float2(0.f, 0.f);
 
   // this CTA's row of the partial-output buffer doubles as the outlier accumulator: cleared here, reduced into by
-  // the outlier rows, read back (after a fence) and completed in the epilogue
+  // the outlier rows, read back (after a fence) and completed in the epilogue.  Only this CTA's heads are touched.
   float* obase = p.out_o + (int64_t)blockIdx.x * hidden;
   if (p.outliers != nullptr) {
-    for (int i = tid; i < hidden; i += kNThreads) obase[i] = 0.f;
+    for (int i = h0 * kHeadDim + tid; i < (h0 + Hg) * kHeadDim; i += kNThreads) obase[i] = 0.f;
     __threadfence();   // the clears reach L2 before any reduction (ordered by the __syncthreads below)
   }
   if (tid == 0) {
@@ -220,10 +227,10 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
     const int64_t t0 = (tile0 + it) * kNT;
     mbar_expect_tx(&s_bar[s], lay.stage_bytes);
     unsigned char* dst = smem + (size_t)s * lay.stage_bytes;
-    for (int b = 0; b < nbox; ++b) tma_load_2d(dst + (size_t)b * p.box_rows * 128, &tmap, &s_bar[s], (int)t0, b * p.box_rows);
+    for (int b = 0; b < nbox; ++b) tma_load_2d(dst + (size_t)b * p.box_rows * 128, &tmap, &s_bar[s], (int)t0, h0 * W + b * p.box_rows);
   };
-  // weights: H*32 (head, token) values per tile -> 2 per thread at H = 32 (up to 4 at H = 64)
-  const int n_w = p.H * kNT;
+  // weights: Hg*32 (head, token) values per tile -> 2 per thread at Hg = 32 (up to 4 at Hg = 64)
+  const int n_w = Hg * kNT;
   constexpr int NW = 4;
   float wpre[NW], wspre[NW], offpre[NW];
   float lacc[NW], oacc_off[NW];
@@ -241,8 +248,8 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
       if (e < n_w) {
         const int h = e >> 5, tl = e & 31;
         if (t0 + tl < L_eff) {
-          w_s[i] = p.score[(int64_t)h * p.score_stride + t0 + tl];
-          w_m[i] = p.gmax[h];
+          w_s[i] = p.score[(int64_t)(h0 + h) * p.score_stride + t0 + tl];
+          w_m[i] = p.gmax[h0 + h];
           w_a[i] = *reinterpret_cast<const float2*>(p.v_aff + 2 * (t0 + tl));
         }
       }
@@ -264,8 +271,8 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
       const int e = tid + i * kNThreads;
       if (e < n_w) {
         const int h = e >> 5, tl = e & 31;
-        s_w[(buf * p.H + h) * kNWStride + tl] = wpre[i];
-        s_ws[(buf * p.H + h) * kNWsStride + tl] = wspre[i];
+        s_w[(buf * Hg + h) * kNWStride + tl] = wpre[i];
+        s_ws[(buf * Hg + h) * kNWsStride + tl] = wspre[i];
       }
     }
   };
@@ -278,6 +285,8 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
   float opre_v[NO];
   int opre_i[NO];
   const bool has_out = p.outliers != nullptr;
+  // a V outlier row spans all heads: a head-split CTA applies the entries of its own heads only
+  auto own_head = [&](int idx) { return !SPLIT || (unsigned)((idx >> 7) - h0) < (unsigned)Hg; };
   auto load_outliers = [&](int it) {
     const int64_t t0 = (tile0 + it) * kNT;
 #pragma unroll
@@ -311,7 +320,7 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
     const int s = it % S;
     mbar_wait(&s_bar[s], (uint32_t)((it / S) & 1));
     const unsigned char* stage = smem + (size_t)s * lay.stage_bytes;
-    const float* wsbuf = s_ws + (it & 1) * p.H * kNWsStride;
+    const float* wsbuf = s_ws + (it & 1) * Hg * kNWsStride;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       if (u_on[i]) {
@@ -326,24 +335,22 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
       }
     }
     if (has_out) {
-      const float* wbuf = s_w + (it & 1) * p.H * kNWStride;
+      const float* wbuf = s_w + (it & 1) * Hg * kNWStride;
 #pragma unroll
       for (int j = 0; j < kNTokPerWarp; ++j) {
         const int tl = warp + j * (kNThreads / 32);
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           const float v = opre_v[2 * j + r];
-          if (v != 0.f) {
-            const int idx = opre_i[2 * j + r];
-            red_add_f32(obase + idx, v * wbuf[(idx >> 7) * kNWStride + tl]);
-          }
+          const int idx = opre_i[2 * j + r];
+          if (v != 0.f && own_head(idx)) red_add_f32(obase + idx, v * wbuf[((idx >> 7) - h0) * kNWStride + tl]);
         }
         for (int k = lane + 64; k < p.n_out; k += 32) {   // n_out > 64: unprefetched tail
           const int64_t t = (tile0 + it) * kNT + tl;
           if (t < L_eff) {
             const float v = p.outliers[t * p.n_out + k];
             const int idx = p.outlier_idx[t * p.n_out + k];
-            if (v != 0.f) red_add_f32(obase + idx, v * wbuf[(idx >> 7) * kNWStride + tl]);
+            if (v != 0.f && own_head(idx)) red_add_f32(obase + idx, v * wbuf[((idx >> 7) - h0) * kNWStride + tl]);
           }
         }
       }
@@ -354,9 +361,9 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
   __syncthreads();
 
   // ---- epilogue: per-head scalars (denominator, offset term), then the partial output -----------------------------
-  float* s_l = s_w;            // [H]
-  float* s_off = s_w + p.H;    // [H]
-  for (int i = tid; i < 2 * p.H; i += kNThreads) s_w[i] = 0.f;
+  float* s_l = s_w;            // [Hg]
+  float* s_off = s_w + Hg;     // [Hg]
+  for (int i = tid; i < 2 * Hg; i += kNThreads) s_w[i] = 0.f;
   __syncthreads();
 #pragma unroll
   for (int i = 0; i < NW; ++i) {
@@ -366,7 +373,7 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
     if (e < n_w && lane == 0) { atomicAdd(&s_l[e >> 5], a); atomicAdd(&s_off[e >> 5], b); }
   }
   __syncthreads();
-  for (int i = tid; i < p.H; i += kNThreads) p.out_l[(int64_t)blockIdx.x * p.H + i] = s_l[i];
+  for (int i = tid; i < Hg; i += kNThreads) p.out_l[(int64_t)blockIdx.x * p.H + h0 + i] = s_l[i];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     if (u_on[i]) {
@@ -375,7 +382,7 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
 #pragma unroll
       for (int k = 0; k < 2 * NP; ++k) {
         if (k < nch) {
-          const int j = u_head[i] * kHeadDim + u_ch0[i] + k;
+          const int j = (h0 + u_head[i]) * kHeadDim + u_ch0[i] + k;
           const float v = (k & 1) ? acc[i][k >> 1].y : acc[i][k >> 1].x;
           obase[j] = v + hoff + (has_out ? __ldcg(obase + j) : 0.f);
         }
@@ -387,38 +394,61 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
 constexpr uint32_t kVNSmemBudget = 227u * 1024u;
 int num_sms_cached();
 
+// ring stages that fit next to the table for a slab of Hg heads (largest first); 0 when not even two do
 template <int BITS>
-static int launch_vn(VNParams p, const int32_t* cache, int* n_cta_out, cudaStream_t st) {
+static int vn_stages(int Hg, VNSmem* lay) {
   using C = VNCfg<BITS>;
-  const int rows = p.H * C::W;
-  int S = kNMaxStages;
-  VNSmem lay{};
-  for (; S >= 2; --S) {
-    lay = vn_smem_layout(rows, C::TABN, p.H, S);
-    if (lay.total + 1024u <= kVNSmemBudget) break;
+  for (int S = kNMaxStages; S >= 2; --S) {
+    *lay = vn_smem_layout(Hg * C::W, C::TABN, Hg, S);
+    if (lay->total + 1024u <= kVNSmemBudget) return S;
   }
-  if (S < 2) return KVQ_E_UNSUPPORTED;
-  p.n_stages = S;
+  return 0;
+}
+
+template <int BITS, bool SPLIT>
+static int launch_vn_kernel(const CUtensorMap& tmap, const VNParams& p, dim3 grid, uint32_t smem, cudaStream_t st) {
   static PerDeviceOnce attr_once;
   bool& attr_done = attr_once.cur();
   if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(v_native_kernel<BITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVNSmemBudget);
+    cudaError_t e = cudaFuncSetAttribute(v_native_kernel<BITS, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVNSmemBudget);
     if (e != cudaSuccess) return (int)e;
     attr_done = true;
   }
+  v_native_kernel<BITS, SPLIT><<<grid, kNThreads, smem, st>>>(tmap, p);
+  KVQ_LAUNCH_CHECK();
+  return 0;
+}
+
+template <int BITS>
+static int launch_vn(VNParams p, const int32_t* cache, int* n_cta_out, cudaStream_t st) {
+  using C = VNCfg<BITS>;
+  // G head groups: 1 while the whole slab fits (every shape up to 4-bit H = 32, 3-bit H = 56, 2-bit H = 64), else 2.
+  // G = 2 always fits for H <= 64: Hg = H/2 <= 32 heads is at most the 7B slab, and H % 4 == 0 keeps Hg even, so
+  // the 3-bit group rows (Hg*12) stay a multiple of 8 for the TMA box below.
+  VNSmem lay{};
+  int G = 1;
+  int S = vn_stages<BITS>(p.H, &lay);
+  if (S < 2) { G = 2; S = vn_stages<BITS>(p.H / G, &lay); }
+  if (S < 2) return KVQ_E_UNSUPPORTED;
+  p.n_stages = S;
+  const int rows = p.H / G * C::W;   // word rows of one head group
   CUtensorMap tmap;
-  // largest TMA box height <= 256 that divides the row count (rows is a multiple of 32)
+  // largest TMA box height <= 256 that divides the group's row count (a multiple of 8); one map over the whole
+  // cache, the kernel offsets the row coordinate by its group's first row
   int nb = (rows + 255) / 256;
   while (rows % nb != 0 || (rows / nb) % 8 != 0) ++nb;
   p.box_rows = rows / nb;
-  int rc = make_cache_tensor_map(&tmap, cache, (uint64_t)rows, (uint64_t)p.Lmax, kNT, (uint32_t)p.box_rows, /*swizzle bytes*/ 128);
+  int rc = make_cache_tensor_map(&tmap, cache, (uint64_t)p.H * C::W, (uint64_t)p.Lmax, kNT, (uint32_t)p.box_rows, /*swizzle bytes*/ 128);
   if (rc != 0) return rc;
+  // token ranges x head groups ~ one CTA per SM; the partial index is the token range
   const int64_t n_tiles = (p.L + kNT - 1) / kNT;
-  const int sms = num_sms_cached();
-  p.tiles_per_cta = (int)((n_tiles + sms - 1) / sms);
+  const int ranges = max(1, num_sms_cached() / G);
+  p.tiles_per_cta = (int)((n_tiles + ranges - 1) / ranges);
   const int n_cta = (int)((n_tiles + p.tiles_per_cta - 1) / p.tiles_per_cta);
-  v_native_kernel<BITS><<<n_cta, kNThreads, lay.total + 1024u, st>>>(tmap, p);
-  KVQ_LAUNCH_CHECK();
+  const dim3 grid(n_cta, G);
+  rc = G == 1 ? launch_vn_kernel<BITS, false>(tmap, p, grid, lay.total + 1024u, st)
+              : launch_vn_kernel<BITS, true>(tmap, p, grid, lay.total + 1024u, st);
+  if (rc != 0) return rc;
   *n_cta_out = n_cta;
   return 0;
 }
