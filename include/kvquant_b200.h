@@ -174,7 +174,12 @@ KVQ_API int kvq_attend_dyn(int bits, const float* q, const int32_t* kcache, cons
  * QuantK/QuantV.forward_fused_sparse (modeling_llama.py:664-751, 1803-1820, 1091-1176): append kernel +
  * .cpu() + torch.topk + gather/mask/sort + row writes, for K and V of one token, in one launch, no host sync.
  *   k_new, v_new: f32 [H*128].  n_each = int(((1-t)/2)*hidden)+1 (21 for 7B): K keeps the n_each largest /
- *   smallest normalised values, V thresholds are the (n_each+1)-th order statistics.
+ *   smallest normalised values, V thresholds are the (n_each+1)-th order statistics.  n_each <= 64.
+ *   Ties: K values equal at the n_each boundary are taken lowest channel first.  The V outliers are the elements
+ *   strictly beyond the thresholds (those packed as the zero-point code); when values equal to a threshold leave
+ *   fewer than n_each on a side, the side is padded with (value 0.0, channel 0), and the row is sorted by channel.
+ *   (The reference's topk row keeps tied elements instead, which then count twice: their dense code is their
+ *   nearest entry, not the zero point -- DESIGN.md section 2.)
  *   klut_sub: LUT used for the K end-entry subtraction (lookup_table2 under Q-Norm), may equal klut.
  *   v_cent: f32 [2^bits] sorted centroids; vlut_tok row `slot` is WRITTEN; v_aff (optional, f32 [Lmax,2]) row
  *   `slot` receives (sf, off); v_cent_deq (optional): Q-Norm centroids cent*normscale+normoffset -- the outlier

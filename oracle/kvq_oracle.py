@@ -75,11 +75,10 @@ def pack_codes(codes: np.ndarray, bits: int) -> np.ndarray:
     elif bits == 2:
         np.add.at(out, j // 16, c << ((j % 16) * 2).astype(np.uint32)[:, None])
     elif bits == 3:
-        loc = j % 32
-        base = (j // 32) * 3
-        for jj in range(hidden):
-            l, b = int(loc[jj]), int(base[jj])
-            v = c[jj]
+        for l in range(32):              # every channel at position l of its 32-group, all groups at once
+            js = j[l::32]
+            b = (js // 32) * 3
+            v = c[js]
             if l == 10:
                 out[b] += (v << np.uint32(30))
                 out[b + 1] += (v >> np.uint32(2))
@@ -108,15 +107,16 @@ def unpack_codes(words: np.ndarray, bits: int) -> np.ndarray:
         return ((w[j // 16] >> ((j % 16) * 2).astype(np.uint32)[:, None]) & 0x3).astype(np.uint8)
     if bits == 3:
         out = np.zeros((hidden, T), dtype=np.uint8)
-        for jj in range(hidden):
-            l, b = jj % 32, (jj // 32) * 3
+        for l in range(32):
+            js = j[l::32]
+            b = (js // 32) * 3
             if l == 10:
                 v = ((w[b] >> np.uint32(30)) & 0x3) | ((w[b + 1] & 0x1) << np.uint32(2))
             elif l == 21:
                 v = ((w[b + 1] >> np.uint32(31)) & 0x1) | ((w[b + 2] & 0x3) << np.uint32(1))
             else:
                 v = (w[b + l // 11] >> np.uint32((3 * l) % 32)) & 0x7
-            out[jj] = v.astype(np.uint8)
+            out[js] = v.astype(np.uint8)
         return out
     raise ValueError(bits)
 
@@ -152,12 +152,16 @@ def build_k_lut(upper, lower, centroids, normscale=None, normoffset=None):
     )
 
 
-def v_token_lut(cent_sorted, hi, lo):
-    """Per-token V LUT (ML.py:1097-1114): sf=(hi-lo)/2, off=(hi+lo)/2 in fp32; LUT = cent*sf + off."""
+def v_token_affine(hi, lo):
+    """(sf, off) = ((hi-lo)/2, (hi+lo)/2) in fp32 (ML.py:1097-1098)."""
     hi = F32(hi)
     lo = F32(lo)
-    off = F32(F32(hi + lo) / F32(2))
-    sf = F32(F32(hi - lo) / F32(2))
+    return F32(F32(hi - lo) / F32(2)), F32(F32(hi + lo) / F32(2))
+
+
+def v_token_lut(cent_sorted, hi, lo):
+    """Per-token V LUT (ML.py:1097-1114): sf=(hi-lo)/2, off=(hi+lo)/2 in fp32; LUT = cent*sf + off."""
+    sf, off = v_token_affine(hi, lo)
     cent = np.asarray(cent_sorted, dtype=np.float32)
     return ((cent * sf).astype(np.float32) + off).astype(np.float32)
 
@@ -199,8 +203,13 @@ def k_outliers_rescaled(k, thr_lower, thr_upper):
 
 
 def _topk_idx(x, k, largest=True):
-    """indices of the k largest / smallest entries (torch.topk; tie order unspecified in torch --
-    a stable sort is used here, ties do not occur in continuous synthetic data)."""
+    """indices of the k largest / smallest entries, equal values lowest index first (stable sort).
+
+    torch.topk, which the reference calls, leaves the order of equal values unspecified.  Lowest index first is the
+    fused append's K rule (kvq_append_kv_fused: among equal normalised values at the n_each boundary the lowest channel
+    is taken), so K rows here are exact with ties.  For V the choice only matters under v_ties="reference": which of
+    several values equal to a threshold land in the row (see v_outlier_row_strict for the fused append's V rule).
+    fp16-valued activations -- what a decode step feeds the append -- produce such ties in a few % of V tokens."""
     x = np.asarray(x)
     order = np.argsort(-x if largest else x, kind="stable")
     return order[:k]
@@ -261,6 +270,36 @@ def v_outlier_row(v, upper_idx, lower_idx, zeropoint_val):
     v = np.asarray(v, dtype=np.float32)
     idx = np.concatenate([upper_idx, lower_idx]).astype(np.int64)
     vals = (v[idx] - F32(zeropoint_val)).astype(np.float32)
+    order = np.argsort(idx, kind="stable")
+    return vals[order], idx[order].astype(np.int32)
+
+
+def v_outlier_row_strict(v, hi, lo, n_each, zeropoint_val):
+    """V outlier row of the fused append (kvq_append_kv_fused), the rule for ties at the thresholds.
+
+    The outliers are the elements strictly beyond the (n_each+1)-th order statistics: v > hi and v < lo -- exactly the
+    elements whose dense code is the zero-point code (append_v_codes), so each element is represented once.  When
+    values equal to a threshold leave fewer than n_each on a side, that side is padded with (0.0, channel 0).
+    Sorted by channel; entries of one channel keep the order upper outliers, upper pads, lower outliers, lower pads.
+
+    The reference (v_outlier_row, v_ties="reference") instead keeps n_each topk indices per side, some of them equal
+    to the threshold.  Such an element's dense code is its nearest LUT entry (the sparse append compares strictly),
+    so it dequantises to LUT_t[code] + (v - LUT_t[zp]): its value is counted twice."""
+    v = np.asarray(v, dtype=np.float32)
+    up = np.nonzero(v > F32(hi))[0]
+    lw = np.nonzero(v < F32(lo))[0]
+    assert len(up) <= n_each and len(lw) <= n_each
+
+    def side(ix):
+        vals = np.zeros(n_each, dtype=np.float32)
+        vals[:len(ix)] = (v[ix] - F32(zeropoint_val)).astype(np.float32)
+        idx = np.zeros(n_each, dtype=np.int64)
+        idx[:len(ix)] = ix
+        return vals, idx
+    uv, ui = side(up)
+    lv, li = side(lw)
+    vals = np.concatenate([uv, lv])
+    idx = np.concatenate([ui, li])
     order = np.argsort(idx, kind="stable")
     return vals[order], idx[order].astype(np.int32)
 
@@ -501,9 +540,14 @@ class OracleCache:
     QuantK/QuantV.forward_fused_sparse do (ML.py:653-751, 1069-1176)."""
 
     def __init__(self, bits, num_heads, max_len, klut, v_cent, include_sparse=True, sparsity_threshold=0.99,
-                 v_norm=None, sparse_v=None):
+                 v_norm=None, sparse_v=None, v_ties="reference"):
         """v_norm = (normscale, normoffset) enables Q-Norm on V (ML.py:1054-1066,1115-1118); K Q-Norm is enabled by
-        klut['lut2'] (ML.py:485-488): packing uses LUT, dequantisation and outlier subtraction use LUT2."""
+        klut['lut2'] (ML.py:485-488): packing uses LUT, dequantisation and outlier subtraction use LUT2.
+        v_ties: which V outlier row a token with values equal to a threshold gets -- "reference" (the reference's topk
+        row, v_outlier_row) or "strict" (the fused append's row, v_outlier_row_strict).  Without such ties both agree."""
+        if v_ties not in ("reference", "strict"):
+            raise ValueError(v_ties)
+        self.v_ties = v_ties
         self.bits = bits
         self.H = num_heads
         self.hidden = num_heads * HEAD_DIM
@@ -519,6 +563,7 @@ class OracleCache:
         self.kwords = np.zeros((W, max_len), dtype=np.int32)
         self.vwords = np.zeros((W, max_len), dtype=np.int32)
         self.vlut = np.zeros((max_len, 2 ** bits), dtype=np.float32)
+        self.vaff = np.zeros((max_len, 2), dtype=np.float32)   # (sf_t, off_t) of each row of vlut
         self.v_norm = v_norm
         self.v_cent2 = None if v_norm is None else ((self.v_cent * F32(v_norm[0])).astype(np.float32) + F32(v_norm[1])).astype(np.float32)
         self.vlut2 = np.zeros((max_len, 2 ** bits), dtype=np.float32) if v_norm is not None else None
@@ -539,15 +584,21 @@ class OracleCache:
             self.k_out[t], self.k_idx[t] = k_outlier_row(k, r, sub, self.n_each)
         if self.sparse_v:
             hi, lo, ui, li = v_thresholds(v, self.n_each)
+            self.vaff[t] = v_token_affine(hi, lo)
             self.vlut[t] = v_token_lut(self.v_cent, hi, lo)
             codes = append_v_codes(v, self.vlut[t], self.bits, lo, hi)
             zrow = self.vlut[t]
             if self.v_norm is not None:   # ML.py:1115-1118, 1149-1152: zero-point taken from the Q-Norm table
                 self.vlut2[t] = v_token_lut(self.v_cent2, hi, lo)
                 zrow = self.vlut2[t]
-            self.v_out[t], self.v_idx[t] = v_outlier_row(v, ui, li, zrow[zero_point_code(self.bits)])
+            zp = zrow[zero_point_code(self.bits)]
+            if self.v_ties == "strict":
+                self.v_out[t], self.v_idx[t] = v_outlier_row_strict(v, hi, lo, self.n_each, zp)
+            else:
+                self.v_out[t], self.v_idx[t] = v_outlier_row(v, ui, li, zp)
         else:
             v = np.asarray(v, dtype=np.float32)
+            self.vaff[t] = v_token_affine(v.max(), v.min())
             self.vlut[t] = v_token_lut(self.v_cent, v.max(), v.min())  # compute_lut (ML.py:318-349)
             codes = append_v_codes(v, self.vlut[t], self.bits)
         self.vwords[:, t] = pack_codes(codes, self.bits)[:, 0]
