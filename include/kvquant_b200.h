@@ -200,6 +200,31 @@ KVQ_API int kvq_append_kv_fused(int bits, int H, int64_t Lmax, int64_t slot, int
                         void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Dequantise slots [start, stop) of a layer cache to fp16 (native op: the cache read back as dense K / V, for
+ * multi-token attention, other attention kernels, or checking the cache on the device).
+ *   out_k / out_v: __half, element (h, t, c) at  h*head_stride + (t-start)*128 + c  (either may be NULL, not both);
+ *   head_stride >= (stop-start)*128 and a multiple of 8; outputs 16-byte aligned (so a slice of a bigger [H, S, 128]
+ *   buffer can be written in place).
+ *   K: klut = the dequantisation table (LUT2 under Q-Norm, as kvq_attend takes it); value = LUT[h,c,code] + the K
+ *      outlier residual of (slot, channel) if present, one fp32 add, then one rounding to fp16.
+ *      rope_cos_sin == NULL -> written pre-RoPE; otherwise rotated at position p = pos_offset + t with the
+ *      kvq_rope_table_build table (rotate-half: k'[c] = cos*k[c] - sin*k[c+64] (c<64), cos*k[c] + sin*k[c-64]
+ *      (c>=64)), so that for a query already rotated at its own position, q . k'[t] is the score kvq_attend computes
+ *      for slot t; the table must cover positions [0, pos_offset + stop).
+ *   V: value = v_cent[code]*sf_t + off_t (one fma; v_cent = the Q-Norm-shifted centroids when V Q-Norm is on, (sf_t,
+ *      off_t) = v_aff row t) + the V outlier residual.  Native V form only (like kvq_attend_dyn).
+ *   k_outliers / v_outliers pairs may be NULL (dense-only cache, or K outliers only); n_out <= 128, even.
+ *   start == stop returns 0 once the sizes are valid, whatever the pointers (an empty output may be NULL), and
+ *   launches nothing.  All offsets are 64-bit.  Two launches (K, V) on `stream`.
+ * ------------------------------------------------------------------------------------------------------------- */
+KVQ_API int kvq_dequant_kv(int bits, int H, int64_t Lmax, int64_t start, int64_t stop,
+                   const int32_t* kcache, const float* klut, const float* k_outliers, const int32_t* k_outlier_idx,
+                   const int32_t* vcache, const float* v_cent, const float* v_aff,
+                   const float* v_outliers, const int32_t* v_outlier_idx, int n_out,
+                   const float* rope_cos_sin, int64_t rope_npos, int pos_offset,
+                   void* out_k, void* out_v, int64_t head_stride, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Uncapped "orig" sparse path, 4-bit only (quant_cuda.cpp:347-399).
  * SpMV halves of ..._opt2_orig: balanced CSR (K; rows = tokens) quant_cuda_kernel.cu:523-614 and CSC (V; cols =
  * tokens) 616-689; the dense half is kvq_k_matvec / kvq_v_matvec with outliers == NULL.

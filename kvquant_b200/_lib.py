@@ -41,6 +41,8 @@ SIGNATURES = {
                                          _p, _p, _p, _p, _p, _p, _p, _p]),
     "kvq_attend_dyn": (_c_int, [_c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int, _c_i64, _c_i64, _p,
                                 _c_i64, _p, _c_i64, _c_f, _c_int, _p, _p, _c_int, _p, _p, _p, _p, _p]),
+    "kvq_dequant_kv": (_c_int, [_c_int, _c_int, _c_i64, _c_i64, _c_i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int,
+                                _p, _c_i64, _c_int, _p, _p, _c_i64, _p]),
     "kvq_p2p_buffer_bytes": (_c_i64, [_c_int, _c_int]),
     "kvq_p2p_alloc": (_c_int, [_p, _c_i64, _p]),
     "kvq_p2p_open": (_c_int, [_p, _p]),

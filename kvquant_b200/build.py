@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libkvquant_b200.so")
-SOURCES = ["kvq_capi.cu", "kvq_append.cu", "kvq_kscore.cu", "kvq_kpair.cu", "kvq_k3.cu", "kvq_kfast.cu", "kvq_kratio.cu", "kvq_vaccum.cu", "kvq_vnative.cu", "kvq_orig.cu", "kvq_decode_ops.cu", "kvq_decode_gemv.cu", "kvq_p2p.cu"]
+SOURCES = ["kvq_capi.cu", "kvq_append.cu", "kvq_kscore.cu", "kvq_kpair.cu", "kvq_k3.cu", "kvq_kfast.cu", "kvq_kratio.cu", "kvq_vaccum.cu", "kvq_vnative.cu", "kvq_orig.cu", "kvq_decode_ops.cu", "kvq_decode_gemv.cu", "kvq_p2p.cu", "kvq_dequant.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",  # H100 only; no fallback archs, no fast-math
     "-O3", "-std=c++17", "-lineinfo",

@@ -278,6 +278,114 @@ class LayerCache:
             rope_h.data_ptr() if fast else None, torch.cuda.current_stream().cuda_stream), "kvq_attend_dyn")
         return out
 
+    def _kv_out(self, t, n, name):
+        """Caller-supplied fp16 [H, n, 128] output, possibly a view into a larger [H, S, 128] buffer: tokens and
+        channels packed (stride (S*128, 128, 1)), on this cache's device, 16-byte aligned.  Returns the head stride."""
+        if not isinstance(t, torch.Tensor):
+            raise TypeError("%s must be a torch.Tensor" % name)
+        if t.dtype != torch.float16:
+            raise TypeError("%s must be torch.float16, got %s" % (name, t.dtype))
+        if t.device != self.device:
+            raise ValueError("%s is on %s, the cache lives on %s" % (name, t.device, self.device))
+        if tuple(t.shape) != (self.H, n, HEAD_DIM):
+            raise ValueError("%s has shape %s, expected %s" % (name, tuple(t.shape), (self.H, n, HEAD_DIM)))
+        if t.stride(2) != 1 or t.stride(1) != HEAD_DIM or t.stride(0) < n * HEAD_DIM:
+            raise ValueError("%s must have strides (S*128, 128, 1) with S >= %d, got %s" % (name, n, t.stride()))
+        if t.data_ptr() % 16 or t.stride(0) % 8:
+            raise ValueError("%s must be 16-byte aligned with a head stride that is a multiple of 8" % name)
+        return t.stride(0)
+
+    @_on_cache_device
+    def dequantize(self, start=0, stop=None, rope_theta=None, out_k=None, out_v=None):
+        """Slots [start, stop) of the cache as fp16 K and V, each [H, stop-start, 128] (one device pass, kvq_dequant_kv).
+
+        K is the dequantised value (dequantisation table plus outlier residual); with rope_theta=None it is pre-RoPE,
+        otherwise rotated at the absolute positions n_sink + pos_base + t -- the positions attend() uses -- so that
+        q . k[t] for a query rotated at its own position is the score attend() computes for slot t.  V is
+        v_cent[code]*sf_t + off_t plus its outlier residual.  out_k / out_v may be views into larger [H, S, 128]
+        buffers (stride (S*128, 128, 1)), each with its own S; an output not given is allocated.  An empty range
+        returns empty outputs.  With both outputs given, and a rope table that already covers the range, the call
+        allocates nothing and can be captured in a CUDA graph."""
+        if not self.use_native_v:
+            raise NotImplementedError("dequantize reads the native V form (use_native_v=True)")
+        stop = self.len if stop is None else int(stop)
+        start = int(start)
+        if not 0 <= start <= stop:
+            raise ValueError("need 0 <= start <= stop, got start=%d stop=%d" % (start, stop))
+        if stop > self.len:
+            raise ValueError("stop=%d is past the %d cached tokens" % (stop, self.len))
+        n = stop - start
+        if out_k is None:
+            out_k = torch.empty((self.H, n, HEAD_DIM), dtype=torch.float16, device=self.device)
+        if out_v is None:
+            out_v = torch.empty((self.H, n, HEAD_DIM), dtype=torch.float16, device=self.device)
+        sk, sv = self._kv_out(out_k, n, "out_k"), self._kv_out(out_v, n, "out_v")
+        if n == 0:
+            return out_k, out_v
+        pos_offset = self.n_sink + self.pos_base
+        rope, npos = None, 0
+        if rope_theta is not None:
+            rope, _, npos = qc.rope_tables(self.device, rope_theta, stop + pos_offset)
+
+        def run(ok, ov, stride):
+            _lib.check(self.lib.kvq_dequant_kv(
+                self.bits, self.H, self.Lmax, start, stop,
+                self.kcache.data_ptr(), self.klut_deq.data_ptr(), *self._out_ptrs("k"),
+                self.vcache.data_ptr(), self.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._out_ptrs("v"),
+                self.n_out, rope.data_ptr() if rope is not None else None, npos, pos_offset,
+                ok, ov, stride, torch.cuda.current_stream().cuda_stream), "kvq_dequant_kv")
+        # one head stride per call: outputs with different strides are written by one call each (K and V are separate
+        # launches either way)
+        if sk == sv:
+            run(out_k.data_ptr(), out_v.data_ptr(), sk)
+        else:
+            run(out_k.data_ptr(), None, sk)
+            run(None, out_v.data_ptr(), sv)
+        return out_k, out_v
+
+    @_on_cache_device
+    def attend_chunk(self, q, k, v, rope_theta=10000.0):
+        """Causal attention of a T-token chunk placed right after the cached tokens (a follow-up prompt).
+
+        q: f32 [T, H, 128], token i already rotated at position P0 + i, P0 = n_sink + pos_base + len.
+        k: f32 [T, hidden] pre-RoPE keys and v: f32 [T, hidden] values of the chunk, as append() takes them.
+        Chunk token i attends over the fp16 sinks (when set), all `len` quantised slots (dequantised and rotated) and
+        chunk tokens 0..i; the chunk's keys are rotated with the same table, and its keys and values rounded to fp16,
+        as a prefill runs attention on the prompt's fp16 K/V.  Scale 1/sqrt(128).  Returns f32 [T, H, 128].
+
+        The cache is NOT modified: append the chunk's tokens afterwards.  The call materialises K and V for every
+        position, 2*H*(n_sink + len + T)*128 fp16 values (2 GiB for 32 heads at 128K tokens), and hands them to
+        torch.nn.functional.scaled_dot_product_attention."""
+        if q.dim() != 3 or q.shape[1:] != (self.H, HEAD_DIM) or q.shape[0] < 1:
+            raise ValueError("q must be [T, %d, %d] with T >= 1, got %s" % (self.H, HEAD_DIM, tuple(q.shape)))
+        T = q.shape[0]
+        for t, name in ((q, "q"), (k, "k"), (v, "v")):
+            self._vec(t, T * self.hidden, name)
+        if tuple(k.shape) != (T, self.hidden) or tuple(v.shape) != (T, self.hidden):
+            raise ValueError("k and v must be [%d, %d]" % (T, self.hidden))
+        L = self.len
+        ns = self.n_sink if self.sink_k is not None else 0
+        S = ns + L + T
+        p0 = self.n_sink + self.pos_base + L
+        kbuf = torch.empty((1, self.H, S, HEAD_DIM), dtype=torch.float16, device=self.device)
+        vbuf = torch.empty_like(kbuf)
+        if ns:
+            kbuf[0, :, :ns] = self.sink_k.transpose(1, 2)
+            vbuf[0, :, :ns] = self.sink_v
+        if L:
+            self.dequantize(0, L, rope_theta, out_k=kbuf[0, :, ns:ns + L], out_v=vbuf[0, :, ns:ns + L])
+        rope, _, _ = qc.rope_tables(self.device, rope_theta, p0 + T)
+        cos, sin = rope[:, p0:p0 + T, 0].t()[:, None, :], rope[:, p0:p0 + T, 1].t()[:, None, :]   # [T, 1, 64]
+        kc = k.view(T, self.H, HEAD_DIM)
+        lo, hi = kc[..., :HEAD_DIM // 2], kc[..., HEAD_DIM // 2:]
+        kbuf[0, :, ns + L:, :HEAD_DIM // 2] = (cos * lo - sin * hi).transpose(0, 1)
+        kbuf[0, :, ns + L:, HEAD_DIM // 2:] = (cos * hi + sin * lo).transpose(0, 1)
+        vbuf[0, :, ns + L:] = v.view(T, self.H, HEAD_DIM).transpose(0, 1)
+        mask = torch.arange(S, device=self.device)[None, :] <= (ns + L + torch.arange(T, device=self.device))[:, None]
+        out = torch.nn.functional.scaled_dot_product_attention(
+            q.transpose(0, 1)[None].half(), kbuf, vbuf, attn_mask=mask, scale=1.0 / math.sqrt(HEAD_DIM))
+        return out[0].transpose(0, 1).float().contiguous()
+
     def bytes_per_token(self):
         """Algorithmic HBM bytes one decode step reads per cached token (SURVEY.md 8d formula)."""
         b = 2 * self.H * HEAD_DIM * self.bits // 8 + 4 * 2 ** self.bits
