@@ -102,6 +102,8 @@ KVQ_API int kvq_rope_table_build_half(void* rope_half, float theta, int64_t n_po
  * kvq_v_matvec replaces ..._transposed_mha_batched_fused_opt (quant_cuda.cpp:214-224; kernel 3211-3433) and ..._opt2
  * (quant_cuda.cpp:226-238; + SPMV_ATOMIC_BALANCED 436-470):
  *   mul[b,h,c] += sum_t (LUT[t,code] (+) outlier) * score[b,h,t].   score f32 [B,H,L]; mul f32 [B,H,128].
+ *   Every H <= 64 with H % 4 == 0 at bits 2-4 (shapes whose all-heads slab does not fit shared memory -- 4-bit
+ *   H >= 48, 3-bit H >= 60 -- run as two head groups).
  * Requires Lmax % 4 == 0 and a 16-byte aligned cache (TMA row pitch).
  * ------------------------------------------------------------------------------------------------------------- */
 KVQ_API int kvq_k_matvec(int bits, const float* q, const int32_t* cache, float* mul, const float* lut,
@@ -119,6 +121,7 @@ KVQ_API int kvq_v_matvec(int bits, const float* score, const int32_t* cache, flo
  * V side: either the reference's materialised per-token LUT (vlut_tok f32 [Lmax,2^bits]) or -- faster -- the
  * sorted centroids v_cent f32 [2^bits] plus the per-token affine map v_aff f32 [Lmax,2] = (sf_t, off_t) with
  * LUT_t[i] = v_cent[i]*sf_t + off_t (what kvq_append_kv_fused writes); when both are given the affine form is used.
+ * Both V forms accept every H <= 64 with H % 4 == 0 at bits 2-4.
  * scratch: device buffer of kvq_attend_scratch_bytes(H, L) bytes.
  * sink_k: f16 [H,128,n_sink] post-RoPE keys, sink_v: f16 [H,n_sink,128] (modeling_llama.py:1464-1466), or NULL.
  * out: f32 [H,128].  out_lse (optional): f32 [H], log-sum-exp of the scaled scores over this call's tokens.

@@ -13,8 +13,12 @@
 //
 // Design (DESIGN.md section 4.2):
 //   * one CTA streams a contiguous token range for ALL heads: the [H*W rows x 32 tokens] code slab of a tile is
-//     fetched by TMA (cp.async.bulk.tensor.2d, 128B swizzle) into a 2-4 stage shared-memory ring behind mbarriers,
-//     together with the tile's per-token LUT rows (cp.async.bulk); nothing is re-read;
+//     fetched by TMA (cp.async.bulk.tensor.2d, 128B swizzle, boxes of 32 rows) into a 2-4 stage shared-memory ring
+//     behind mbarriers, together with the tile's per-token LUT rows (cp.async.bulk); nothing is re-read;
+//   * head split: where the whole slab does not fit shared memory next to the weights and the outlier accumulator
+//     (4-bit H >= 48, 3-bit H >= 60), the grid gains a second dimension of G = 2 head groups and CTA (r, g) streams
+//     only heads [g*H/2, (g+1)*H/2) of token range r, as the native kernel does (kvq_vnative.cu).  The two CTAs of a
+//     range write disjoint heads of the same partial row (fused) or of `mul` (legacy);
 //   * thread = packed word row (8 / 11 / 8 channels): channels stay in registers for the whole range, so there is
 //     no cross-thread reduction per tile (the reference transposes through a 43.5 KB smem tile with 5 barriers
 //     per 128 tokens and finishes with 128 global atomics per block);
@@ -34,6 +38,8 @@ constexpr int kVT = 32;        // tokens per stage
 constexpr int kVMaxStages = 4;
 constexpr int kVMaxWPre = 4;   // prefetched weights per thread  (H*32/512 <= 4  -> H <= 64)
 constexpr int kVMaxOPre = 4;   // prefetched outlier entries per thread (32*n_out/512 <= 4 -> n_out <= 64)
+constexpr int kVBoxRows = 32;  // packed-word rows per TMA box
+constexpr uint32_t kVBoxBytes = kVBoxRows * kVT * 4;   // 4 KiB: a box lands 1024-aligned, as the 128B swizzle needs
 
 struct VParams {
   const float* score;        // [H, score_stride]: legacy = probabilities; fused = scaled scores
@@ -53,18 +59,23 @@ template <int BITS> struct VCfg {
   static constexpr int CH = (BITS == 3) ? 11 : 8;  // channels per thread-unit
 };
 
-// smem carve-up (all offsets from a 1024-aligned base)
+// smem carve-up (all offsets from a 1024-aligned base) for a CTA of Hg heads, rows = Hg*W packed-word rows.
+// The stage holds whole 32-row boxes: the number of boxes issued and the bytes a stage's mbarrier expects both come
+// from nbox (3-bit rows = 12*Hg is not a multiple of 32 when Hg % 8 == 4; the rows of the last box past the group
+// are another group's or, past the tensor, zero-filled by TMA -- counted either way, never read).
 struct VSmem {
-  uint32_t stage_bytes;  // codes per stage (rows*128)
+  int nbox;              // 32-row TMA boxes per stage
+  uint32_t stage_bytes;  // codes per stage (nbox * 4 KiB)
   uint32_t off_lut, off_w, off_oacc, off_bar, total;
 };
-__host__ __device__ inline VSmem v_smem_layout(int rows, int N, int H, int n_stages) {
+__host__ __device__ inline VSmem v_smem_layout(int rows, int N, int Hg, int n_stages) {
   VSmem s;
-  s.stage_bytes = (uint32_t)rows * 128u;
+  s.nbox = (rows + kVBoxRows - 1) / kVBoxRows;
+  s.stage_bytes = (uint32_t)s.nbox * kVBoxBytes;
   s.off_lut = s.stage_bytes * n_stages;
   s.off_w = s.off_lut + (uint32_t)n_stages * kVT * N * 4;
-  s.off_oacc = s.off_w + 2u * H * kVT * 4;
-  s.off_bar = s.off_oacc + (uint32_t)H * kHeadDim * 4;
+  s.off_oacc = s.off_w + 2u * Hg * kVT * 4;
+  s.off_bar = s.off_oacc + (uint32_t)Hg * kHeadDim * 4;
   s.total = s.off_bar + 8u * kVMaxStages;
   return s;
 }
@@ -111,25 +122,28 @@ __device__ __forceinline__ void v_tile_unit(const unsigned char* stage, uint32_t
   }
 }
 
-template <int BITS>
+// SPLIT: gridDim.y head groups (see the head split above); SPLIT = false is the whole-slab launch with h0 = 0
+template <int BITS, bool SPLIT>
 __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_constant__ CUtensorMap tmap, const VParams p) {
   using C = VCfg<BITS>;
   constexpr int N = C::N, W = C::W, CH = C::CH;
   extern __shared__ unsigned char smem_raw[];
   // 128B-swizzled TMA boxes need a 1024-byte aligned base
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int rows = p.H * W;
-  const VSmem lay = v_smem_layout(rows, N, p.H, p.n_stages);
+  const int Hg = SPLIT ? p.H / (int)gridDim.y : p.H;     // heads of this CTA: [h0, h0 + Hg)
+  const int h0 = SPLIT ? (int)blockIdx.y * Hg : 0;
+  const int rows = Hg * W;
+  const VSmem lay = v_smem_layout(rows, N, Hg, p.n_stages);
   float* s_lut = reinterpret_cast<float*>(smem + lay.off_lut);   // [n_stages][32][N]
-  float* s_w = reinterpret_cast<float*>(smem + lay.off_w);       // [2][H][32]
-  float* s_oacc = reinterpret_cast<float*>(smem + lay.off_oacc); // [H*128]
+  float* s_w = reinterpret_cast<float*>(smem + lay.off_w);       // [2][Hg][32]
+  float* s_oacc = reinterpret_cast<float*>(smem + lay.off_oacc); // [Hg*128]
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem + lay.off_bar);
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int S = p.n_stages;
   const int hidden = p.H * kHeadDim;
 
-  // ---- thread -> unit mapping (up to 2 units per thread) ---------------------------------------------------
+  // ---- thread -> unit mapping (up to 2 units per thread); u_head is relative to h0 ---------------------------
   // 4-bit: unit = word row (8 channels).  2-bit: unit = half a word row (8 channels).
   // 3-bit: warp-uniform SUB = warp % 3; unit = (32-channel group gi, SUB): row 3*gi+SUB (11/11/10 channels).
   int u_row[2], u_head[2], u_ch0[2], u_part[2];
@@ -138,7 +152,7 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
   if constexpr (BITS == 3) {
     sub = warp % 3;
     const int tri = warp / 3;            // 5 full warp-triples in 16 warps (warp 15 idles)
-    const int ngroups = p.H * 4;
+    const int ngroups = Hg * 4;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int gi = tri * 32 + lane + i * 160;
@@ -149,7 +163,7 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
       u_part[i] = 0;
     }
   } else {
-    const int nunits = p.H * 16;
+    const int nunits = Hg * 16;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int u = tid + i * kVThreads;
@@ -162,10 +176,10 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int r = u_on[i] ? u_row[i] : 0;
-    r_off[i] = (uint32_t)(r >> 5) * 4096u + (uint32_t)(r & 31) * 128u;
+    r_off[i] = (uint32_t)r * 128u;   // boxes of 32 rows back to back: row r sits at r*128 inside the stage
     r_swz[i] = (uint32_t)(r & 7);
     const int r2 = (r + 1 < rows) ? r + 1 : r;
-    r_off2[i] = (uint32_t)(r2 >> 5) * 4096u + (uint32_t)(r2 & 31) * 128u;
+    r_off2[i] = (uint32_t)r2 * 128u;
     r_swz2[i] = (uint32_t)(r2 & 7);
   }
   float acc[2][CH];
@@ -174,7 +188,7 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
 #pragma unroll
     for (int k = 0; k < CH; ++k) acc[i][k] = 0.f;
 
-  for (int i = tid; i < hidden; i += kVThreads) s_oacc[i] = 0.f;
+  for (int i = tid; i < Hg * kHeadDim; i += kVThreads) s_oacc[i] = 0.f;
   if (tid == 0) {
     for (int s = 0; s < S; ++s) mbar_init(&s_bar[s], 1);
     mbar_fence_init();
@@ -184,7 +198,6 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
   const int64_t n_tiles_total = (p.L + kVT - 1) / kVT;
   const int64_t tile0 = (int64_t)blockIdx.x * p.tiles_per_cta;
   const int ntiles = (int)max((int64_t)0, min((int64_t)p.tiles_per_cta, n_tiles_total - tile0));
-  const int nbox = rows >> 5;
 
   auto issue_tile = [&](int it) {  // thread 0 only
     const int s = it % S;
@@ -192,11 +205,12 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
     const uint32_t lut_bytes = (uint32_t)min((int64_t)kVT, p.Lmax - t0) * N * 4;  // never read past the LUT allocation
     mbar_expect_tx(&s_bar[s], lay.stage_bytes + lut_bytes);
     unsigned char* dst = smem + (size_t)s * lay.stage_bytes;
-    for (int b = 0; b < nbox; ++b) tma_load_2d(dst + b * 4096, &tmap, &s_bar[s], (int)t0, b * 32);
+    for (int b = 0; b < lay.nbox; ++b)
+      tma_load_2d(dst + b * kVBoxBytes, &tmap, &s_bar[s], (int)t0, h0 * W + b * kVBoxRows);
     bulk_load_1d(s_lut + s * kVT * N, p.lut_tok + t0 * N, lut_bytes, &s_bar[s]);
   };
   // weights of a tile: exp(s - max) in fused mode, the given probabilities otherwise; 0 beyond L
-  const int n_w = p.H * kVT;  // values per tile
+  const int n_w = Hg * kVT;  // values per tile
   float wpre[kVMaxWPre];
   auto load_weights = [&](int it) {
     const int64_t t0 = (tile0 + it) * kVT;
@@ -207,8 +221,8 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
       if (e < n_w) {
         const int h = e >> 5, tl = e & 31;
         if (t0 + tl < p.L) {
-          w = p.score[(int64_t)h * p.score_stride + t0 + tl];
-          if (p.fused) w = __expf(w - p.gmax[h]);
+          w = p.score[(int64_t)(h0 + h) * p.score_stride + t0 + tl];
+          if (p.fused) w = __expf(w - p.gmax[h0 + h]);
         }
       }
       wpre[i] = w;
@@ -224,6 +238,8 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
   float opre_v[kVMaxOPre];
   int opre_i[kVMaxOPre];
   const bool has_out = p.outliers != nullptr;
+  // a V outlier row spans all heads: a head-split CTA applies the entries of its own heads only
+  auto own_head = [&](int idx) { return !SPLIT || (unsigned)((idx >> 7) - h0) < (unsigned)Hg; };
   auto load_outliers = [&](int it) {
     const int64_t t0 = (tile0 + it) * kVT;
     const int ntok = (int)min((int64_t)kVT, p.L - t0);
@@ -261,6 +277,16 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
     mbar_wait(&s_bar[s], (uint32_t)((it / S) & 1));
     const unsigned char* stage = smem + (size_t)s * lay.stage_bytes;
     const float* lut_tile = s_lut + s * kVT * N;
+    {
+      // the allocation's last tile: LUT rows past Lmax were not loaded (issue_tile) and the stage may still hold
+      // whatever an earlier kernel left in shared memory -- a NaN there would survive its zero weight.  Clear them
+      // (CTA-uniform branch; this is the last tile any CTA streams, so no later copy lands on these rows)
+      const int64_t t0 = (tile0 + it) * kVT;
+      if (t0 + kVT > p.Lmax) {
+        for (int i = (int)(p.Lmax - t0) * N + tid; i < kVT * N; i += kVThreads) s_lut[s * kVT * N + i] = 0.f;
+        __syncthreads();
+      }
+    }
     const float* wbuf = s_w + (it & 1) * n_w;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -282,16 +308,16 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
 #pragma unroll
       for (int i = 0; i < kVMaxOPre; ++i) {
         const int e = tid + i * kVThreads;
-        if (e < total && opre_v[i] != 0.f) {
-          const int idx = opre_i[i];
+        if (e < total && opre_v[i] != 0.f && own_head(opre_i[i])) {
+          const int idx = opre_i[i] - h0 * kHeadDim;
           const int tl = e / p.n_out;
           atomicAdd(&s_oacc[idx], opre_v[i] * wbuf[(idx >> 7) * kVT + tl]);
         }
       }
       for (int e = tid + kVMaxOPre * kVThreads; e < total; e += kVThreads) {  // n_out > 64: unprefetched tail
         const float v = p.outliers[t0 * p.n_out + e];
-        const int idx = p.outlier_idx[t0 * p.n_out + e];
-        if (v != 0.f) atomicAdd(&s_oacc[idx], v * wbuf[(idx >> 7) * kVT + e / p.n_out]);
+        const int idx = p.outlier_idx[t0 * p.n_out + e] - h0 * kHeadDim;
+        if (v != 0.f && own_head(idx + h0 * kHeadDim)) atomicAdd(&s_oacc[idx], v * wbuf[(idx >> 7) * kVT + e / p.n_out]);
       }
     }
     if (more) {
@@ -304,8 +330,8 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
 
   // ---- epilogue --------------------------------------------------------------------------------------------
   if (p.fused) {
-    float* s_l = s_w;  // reuse: [H]
-    for (int i = tid; i < p.H; i += kVThreads) s_l[i] = 0.f;
+    float* s_l = s_w;  // reuse: [Hg]
+    for (int i = tid; i < Hg; i += kVThreads) s_l[i] = 0.f;
     __syncthreads();
 #pragma unroll
     for (int i = 0; i < kVMaxWPre; ++i) {
@@ -316,7 +342,7 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
       }
     }
     __syncthreads();
-    for (int i = tid; i < p.H; i += kVThreads) p.out_l[(int64_t)blockIdx.x * p.H + i] = s_l[i];
+    for (int i = tid; i < Hg; i += kVThreads) p.out_l[(int64_t)blockIdx.x * p.H + h0 + i] = s_l[i];
   }
   float* obase = p.fused ? (p.out + (int64_t)blockIdx.x * hidden) : p.out;
 #pragma unroll
@@ -328,8 +354,8 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
         if (k < nch) {
           const int j = u_head[i] * kHeadDim + u_ch0[i] + k;
           const float v = acc[i][k] + s_oacc[j];
-          if (p.fused) obase[j] = v;
-          else atomicAdd(&obase[j], v);
+          if (p.fused) obase[h0 * kHeadDim + j] = v;
+          else atomicAdd(&obase[h0 * kHeadDim + j], v);
         }
       }
     }
@@ -468,35 +494,57 @@ int num_sms_cached() {
 
 constexpr uint32_t kSmemBudget = 227u * 1024u;
 
-// returns number of CTAs launched (>0) or an error (<=0 mapped by caller)
+// ring stages that fit next to the LUT rows, weights and outlier accumulator for a slab of Hg heads (largest
+// first); 0 when not even two do
 template <int BITS>
-static int launch_v(VParams p, const int32_t* cache, int* n_cta_out, cudaStream_t st) {
+static int v_stages(int Hg, VSmem* lay) {
   using C = VCfg<BITS>;
-  const int rows = p.H * C::W;
-  int S = kVMaxStages;
-  VSmem lay{};
-  for (; S >= 2; --S) {
-    lay = v_smem_layout(rows, C::N, p.H, S);
-    if (lay.total + 1024u <= kSmemBudget) break;
+  for (int S = kVMaxStages; S >= 2; --S) {
+    *lay = v_smem_layout(Hg * C::W, C::N, Hg, S);
+    if (lay->total + 1024u <= kSmemBudget) return S;
   }
-  if (S < 2) return KVQ_E_UNSUPPORTED;
-  p.n_stages = S;
+  return 0;
+}
+
+template <int BITS, bool SPLIT>
+static int launch_v_kernel(const CUtensorMap& tmap, const VParams& p, dim3 grid, uint32_t smem, cudaStream_t st) {
   static PerDeviceOnce attr_once;
   bool& attr_done = attr_once.cur();
   if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(v_accum_kernel<BITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget);
+    cudaError_t e = cudaFuncSetAttribute(v_accum_kernel<BITS, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget);
     if (e != cudaSuccess) return (int)e;
     attr_done = true;
   }
-  CUtensorMap tmap;
-  int rc = make_cache_tensor_map(&tmap, cache, (uint64_t)rows, (uint64_t)p.Lmax, kVT, 32, 128);
-  if (rc != 0) return rc;
-  const int64_t n_tiles = (p.L + kVT - 1) / kVT;
-  const int sms = num_sms();
-  p.tiles_per_cta = (int)((n_tiles + sms - 1) / sms);
-  const int n_cta = (int)((n_tiles + p.tiles_per_cta - 1) / p.tiles_per_cta);
-  v_accum_kernel<BITS><<<n_cta, kVThreads, lay.total + 1024u, st>>>(tmap, p);
+  v_accum_kernel<BITS, SPLIT><<<grid, kVThreads, smem, st>>>(tmap, p);
   KVQ_LAUNCH_CHECK();
+  return 0;
+}
+
+// returns 0 and the number of partial rows written (token ranges) in *n_cta_out, or an error
+template <int BITS>
+static int launch_v(VParams p, const int32_t* cache, int* n_cta_out, cudaStream_t st) {
+  using C = VCfg<BITS>;
+  // G head groups: 1 while the whole slab fits (4-bit H <= 44, 3-bit H <= 56, 2-bit H <= 64), else 2.  G = 2 always
+  // fits for H <= 64: Hg = H/2 <= 32 heads is at most the 7B slab.
+  VSmem lay{};
+  int G = 1;
+  int S = v_stages<BITS>(p.H, &lay);
+  if (S < 2) { G = 2; S = v_stages<BITS>(p.H / G, &lay); }
+  if (S < 2) return KVQ_E_UNSUPPORTED;
+  p.n_stages = S;
+  // one map over the whole cache; a head-split CTA offsets the row coordinate by its group's first row
+  CUtensorMap tmap;
+  int rc = make_cache_tensor_map(&tmap, cache, (uint64_t)p.H * C::W, (uint64_t)p.Lmax, kVT, kVBoxRows, 128);
+  if (rc != 0) return rc;
+  // token ranges x head groups ~ one CTA per SM; the partial index is the token range
+  const int64_t n_tiles = (p.L + kVT - 1) / kVT;
+  const int ranges = max(1, num_sms() / G);
+  p.tiles_per_cta = (int)((n_tiles + ranges - 1) / ranges);
+  const int n_cta = (int)((n_tiles + p.tiles_per_cta - 1) / p.tiles_per_cta);
+  const dim3 grid(n_cta, G);
+  rc = G == 1 ? launch_v_kernel<BITS, false>(tmap, p, grid, lay.total + 1024u, st)
+              : launch_v_kernel<BITS, true>(tmap, p, grid, lay.total + 1024u, st);
+  if (rc != 0) return rc;
   *n_cta_out = n_cta;
   return 0;
 }
