@@ -245,6 +245,36 @@ KVQ_API int kvq_dequant_kv(int bits, int H, int64_t Lmax, int64_t start, int64_t
                    void* out_k, void* out_v, int64_t head_stride, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Causal attention of a T-token chunk over [sinks | quantised slots 0..L-1 | the chunk itself], read straight from
+ * the quantised cache (native op: a prompt chunk attended without materialising the cache as fp16 in HBM).
+ *   Chunk token i attends over the n_sink sinks, all L slots and chunk tokens 0..i; scale 1/sqrt(128).
+ *   q: f32 [T, H, 128], row i rotated at its own position pos_offset + L + i; rounded to fp16 once.
+ *   chunk_k / chunk_v: f16 [H, T, 128], keys rotated at pos_offset + L + i, 16-byte aligned (as are q and out).
+ *   Slot operands: K and V of slot t are the fp16 values kvq_dequant_kv writes for it, bit for bit (K rotated at
+ *      pos_offset + t with the kvq_rope_table_build table, which must cover positions [0, pos_offset + L)); same
+ *      tables and outlier rows as kvq_dequant_kv (klut = LUT2 under Q-Norm, v_cent = the Q-Norm-shifted centroids,
+ *      native V form only); either outlier pair may be NULL, n_out <= 128, even.
+ *   sink_k f16 [H, 128, n_sink] (channel-major, post-RoPE), sink_v f16 [H, n_sink, 128], as kvq_attend takes them.
+ *   Tensor cores (mma.sync m16n8k16, fp16 operands, fp32 scores / softmax / output); K/V tiles are dequantised into
+ *   shared memory.  When (T/128) x H CTAs would fill at most half the SMs the slot range is split over several
+ *   CTAs per row block and a second launch merges their partials (kept in scratch) in a fixed order: two identical
+ *   calls return identical bits.
+ *   out: f32 [T, H, 128].  scratch: device buffer of kvq_attend_chunk_scratch_bytes(H, T, L) bytes (non-decreasing in
+ *   T and L; the same on every device).
+ *   T == 0 returns 0 once the sizes are valid, whatever the pointers, and launches nothing; L == 0 attends the sinks
+ *   and the chunk only.  All offsets are 64-bit.  One or two launches on `stream`.
+ * ------------------------------------------------------------------------------------------------------------- */
+KVQ_API int64_t kvq_attend_chunk_scratch_bytes(int H, int64_t T, int64_t L);
+KVQ_API int kvq_attend_chunk(int bits, int H, int64_t Lmax, int64_t L, int64_t T,
+                   const float* q, const void* chunk_k, const void* chunk_v,
+                   const int32_t* kcache, const float* klut, const float* k_outliers, const int32_t* k_outlier_idx,
+                   const int32_t* vcache, const float* v_cent, const float* v_aff,
+                   const float* v_outliers, const int32_t* v_outlier_idx, int n_out,
+                   const float* rope_cos_sin, int64_t rope_npos, int pos_offset,
+                   const void* sink_k, const void* sink_v, int n_sink,
+                   float* out, void* scratch, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Uncapped "orig" sparse path, 4-bit only (quant_cuda.cpp:347-399).
  * SpMV halves of ..._opt2_orig: balanced CSR (K; rows = tokens) quant_cuda_kernel.cu:523-614 and CSC (V; cols =
  * tokens) 616-689; the dense half is kvq_k_matvec / kvq_v_matvec with outliers == NULL.

@@ -366,6 +366,31 @@ class LayerCache:
             run(None, out_v.data_ptr(), sv)
         return out_k, out_v
 
+    def _chunk_check(self, q, k, v):
+        """The argument checks of attend_chunk / attend_chunk_fused; returns T."""
+        if q.dim() != 3 or q.shape[1:] != (self.H, HEAD_DIM) or q.shape[0] < 1:
+            raise ValueError("q must be [T, %d, %d] with T >= 1, got %s" % (self.H, HEAD_DIM, tuple(q.shape)))
+        T = q.shape[0]
+        for t, name in ((q, "q"), (k, "k"), (v, "v")):
+            self._vec(t, T * self.hidden, name)
+        if tuple(k.shape) != (T, self.hidden) or tuple(v.shape) != (T, self.hidden):
+            raise ValueError("k and v must be [%d, %d]" % (T, self.hidden))
+        return T
+
+    def _chunk_kv16(self, k, v, rope_theta, p0, out_k, out_v):
+        """The chunk's keys rotated at positions p0 + i and its values, written as fp16 into out_k / out_v [H, T, 128]
+        (views allowed): the chunk operands both chunk attentions use.  Returns the f32 rope table, covering
+        p0 + T positions."""
+        T = k.shape[0]
+        rope, _, _ = qc.rope_tables(self.device, rope_theta, p0 + T)
+        cos, sin = rope[:, p0:p0 + T, 0].t()[:, None, :], rope[:, p0:p0 + T, 1].t()[:, None, :]   # [T, 1, 64]
+        kc = k.view(T, self.H, HEAD_DIM)
+        lo, hi = kc[..., :HEAD_DIM // 2], kc[..., HEAD_DIM // 2:]
+        out_k[:, :, :HEAD_DIM // 2] = (cos * lo - sin * hi).transpose(0, 1)
+        out_k[:, :, HEAD_DIM // 2:] = (cos * hi + sin * lo).transpose(0, 1)
+        out_v[:] = v.view(T, self.H, HEAD_DIM).transpose(0, 1)
+        return rope
+
     @_on_cache_device
     def attend_chunk(self, q, k, v, rope_theta=10000.0):
         """Causal attention of a T-token chunk placed right after the cached tokens (a follow-up prompt).
@@ -379,14 +404,9 @@ class LayerCache:
         The cache is NOT modified: append the chunk's tokens afterwards with append_chunk(k, v) (one launch, as
         DecoderStage.prefill does).  The call materialises K and V for every
         position, 2*H*(n_sink + len + T)*128 fp16 values (2 GiB for 32 heads at 128K tokens), and hands them to
-        torch.nn.functional.scaled_dot_product_attention."""
-        if q.dim() != 3 or q.shape[1:] != (self.H, HEAD_DIM) or q.shape[0] < 1:
-            raise ValueError("q must be [T, %d, %d] with T >= 1, got %s" % (self.H, HEAD_DIM, tuple(q.shape)))
-        T = q.shape[0]
-        for t, name in ((q, "q"), (k, "k"), (v, "v")):
-            self._vec(t, T * self.hidden, name)
-        if tuple(k.shape) != (T, self.hidden) or tuple(v.shape) != (T, self.hidden):
-            raise ValueError("k and v must be [%d, %d]" % (T, self.hidden))
+        torch.nn.functional.scaled_dot_product_attention.  attend_chunk_fused computes the same attention without
+        materialising the cache."""
+        T = self._chunk_check(q, k, v)
         L = self.len
         ns = self.n_sink if self.sink_k is not None else 0
         S = ns + L + T
@@ -398,17 +418,41 @@ class LayerCache:
             vbuf[0, :, :ns] = self.sink_v
         if L:
             self.dequantize(0, L, rope_theta, out_k=kbuf[0, :, ns:ns + L], out_v=vbuf[0, :, ns:ns + L])
-        rope, _, _ = qc.rope_tables(self.device, rope_theta, p0 + T)
-        cos, sin = rope[:, p0:p0 + T, 0].t()[:, None, :], rope[:, p0:p0 + T, 1].t()[:, None, :]   # [T, 1, 64]
-        kc = k.view(T, self.H, HEAD_DIM)
-        lo, hi = kc[..., :HEAD_DIM // 2], kc[..., HEAD_DIM // 2:]
-        kbuf[0, :, ns + L:, :HEAD_DIM // 2] = (cos * lo - sin * hi).transpose(0, 1)
-        kbuf[0, :, ns + L:, HEAD_DIM // 2:] = (cos * hi + sin * lo).transpose(0, 1)
-        vbuf[0, :, ns + L:] = v.view(T, self.H, HEAD_DIM).transpose(0, 1)
+        self._chunk_kv16(k, v, rope_theta, p0, kbuf[0, :, ns + L:], vbuf[0, :, ns + L:])
         mask = torch.arange(S, device=self.device)[None, :] <= (ns + L + torch.arange(T, device=self.device))[:, None]
         out = torch.nn.functional.scaled_dot_product_attention(
             q.transpose(0, 1)[None].half(), kbuf, vbuf, attn_mask=mask, scale=1.0 / math.sqrt(HEAD_DIM))
         return out[0].transpose(0, 1).float().contiguous()
+
+    @_on_cache_device
+    def attend_chunk_fused(self, q, k, v, rope_theta=10000.0):
+        """attend_chunk() read straight from the quantised cache (kvq_attend_chunk): same arguments, checks, result
+        (f32 [T, H, 128]) and semantics, and the cache is likewise left untouched.
+
+        One tensor-core kernel dequantises each K/V tile of the cached slots into shared memory -- the same fp16
+        values dequantize() writes -- and attends the chunk over it, FlashAttention-2 style.  Extra device memory per
+        call is the chunk's fp16 rotated K and V (2*H*T*128*2 bytes) plus kvq_attend_chunk_scratch_bytes(H, T, len),
+        whatever `len` is: at 1M cached tokens the materialising attend_chunk would need 2*H*1M*128*2 bytes more."""
+        if not self.use_native_v:
+            raise NotImplementedError("attend_chunk_fused reads the native V form (use_native_v=True)")
+        T = self._chunk_check(q, k, v)
+        L = self.len
+        ns = self.n_sink if self.sink_k is not None else 0
+        pos_offset = self.n_sink + self.pos_base
+        kc = torch.empty((self.H, T, HEAD_DIM), dtype=torch.float16, device=self.device)
+        vc = torch.empty_like(kc)
+        rope = self._chunk_kv16(k, v, rope_theta, pos_offset + L, kc, vc)
+        scratch = torch.empty(max(self.lib.kvq_attend_chunk_scratch_bytes(self.H, T, L), 16), dtype=torch.uint8,
+                              device=self.device)
+        out = torch.empty((T, self.H, HEAD_DIM), dtype=torch.float32, device=self.device)
+        _lib.check(self.lib.kvq_attend_chunk(
+            self.bits, self.H, self.Lmax, L, T, q.data_ptr(), kc.data_ptr(), vc.data_ptr(),
+            self.kcache.data_ptr(), self.klut_deq.data_ptr(), *self._out_ptrs("k"),
+            self.vcache.data_ptr(), self.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._out_ptrs("v"),
+            self.n_out, rope.data_ptr(), rope.shape[1], pos_offset,
+            self.sink_k.data_ptr() if ns else None, self.sink_v.data_ptr() if ns else None, ns,
+            out.data_ptr(), scratch.data_ptr(), torch.cuda.current_stream().cuda_stream), "kvq_attend_chunk")
+        return out
 
     def bytes_per_token(self):
         """Algorithmic HBM bytes one decode step reads per cached token (SURVEY.md 8d formula)."""

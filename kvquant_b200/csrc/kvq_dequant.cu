@@ -12,16 +12,17 @@
 //      channel 0 as a pad, whose value 0 is skipped);
 //   4. each thread converts 8 consecutive channels of one token to fp16 and writes them as one 16-byte store --
 //      for rotated K after combining with the partner channels c ^ 64, which step 3 has already completed.
+// The per-element arithmetic of steps 2-4 is kvq_dequant.cuh's, which kvq_chunk.cu calls too.
 #include <cuda_fp16.h>
 
 #include "kvq_common.cuh"
+#include "kvq_dequant.cuh"
 
 namespace kvq {
 
 constexpr int kTile = 32;       // tokens per tile
 constexpr int kGroup = 2;       // heads per CTA (every accepted H is a multiple of 4)
 constexpr int kThreads = 256;
-constexpr int kMaxOutDq = 128;  // outlier row width bound (2 * n_each, n_each <= 64)
 constexpr int kRopePitch = 65;  // float2 per staged cos/sin row (one token); odd pitch spreads the transposing writes
 constexpr int kTP = kHeadDim + 4;  // fp32 tile row pitch (one token of one head)
 
@@ -108,20 +109,8 @@ __global__ void __launch_bounds__(kThreads, 3) dequant_kernel(const DqParams p) 
 #pragma unroll
       for (int k = 0; k < WQ; ++k) w[k] = words[(g * kTile + t) * D::kWPitch + q * WQ + k];
       float* dst = tile + (g * kTile + t) * kTP + q * 32;
-      const float* lut = tab + (g * kHeadDim + q * 32) * D::kLP;
-      float sf = 0.f, off = 0.f;
-      if constexpr (IS_V) { sf = aff[2 * t]; off = aff[2 * t + 1]; }
-#pragma unroll
-      for (int l = 0; l < 32; l += 4) {
-        float x[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint32_t code = code_of<BITS>(w, l + k);
-          if constexpr (IS_V) x[k] = fmaf(tab[code], sf, off);
-          else x[k] = lut[(l + k) * D::kLP + code];
-        }
-        *reinterpret_cast<float4*>(dst + l) = make_float4(x[0], x[1], x[2], x[3]);
-      }
+      if constexpr (IS_V) dq_quarter<BITS, true>(w, tab, 0, aff[2 * t], aff[2 * t + 1], dst);
+      else dq_quarter<BITS, false>(w, tab + (g * kHeadDim + q * 32) * D::kLP, D::kLP, 0.f, 0.f, dst);
     }
     if (p.outliers != nullptr) {
       __syncthreads();
@@ -131,7 +120,7 @@ __global__ void __launch_bounds__(kThreads, 3) dequant_kernel(const DqParams p) 
         const int g = (idx >> 7) - h0;
         if (g >= 0 && g < kGroup) {
           const float v = p.outliers[row0 + i];
-          if (v != 0.f) atomicAdd(&tile[(g * kTile + i / p.n_out) * kTP + (idx & 127)], v);
+          dq_add_outlier(&tile[(g * kTile + i / p.n_out) * kTP + (idx & 127)], v);
         }
       }
     }
@@ -141,27 +130,8 @@ __global__ void __launch_bounds__(kThreads, 3) dequant_kernel(const DqParams p) 
       const int t = gt % kTile, g = gt / kTile;
       if (t >= nt) continue;
       const int c0 = q * 8;
-      const float* src = tile + gt * kTP;
-      const float4 a = *reinterpret_cast<const float4*>(src + c0);
-      const float4 b = *reinterpret_cast<const float4*>(src + c0 + 4);
-      float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-      if constexpr (!IS_V && ROPE) {
-        // k'[c] = cos*k[c] - sin*k[c+64] (c < 64), cos*k[c] + sin*k[c-64] (c >= 64); j = c mod 64
-        const float4 pa = *reinterpret_cast<const float4*>(src + (c0 ^ 64));
-        const float4 pb = *reinterpret_cast<const float4*>(src + (c0 ^ 64) + 4);
-        const float pv[8] = {pa.x, pa.y, pa.z, pa.w, pb.x, pb.y, pb.z, pb.w};
-        const float sgn = c0 < 64 ? -1.f : 1.f;
-        const float2* row = cs + t * kRopePitch + (c0 & 63);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const float2 r = row[k];
-          v[k] = r.x * v[k] + sgn * (r.y * pv[k]);
-        }
-      }
-      uint4 o;
-      __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) oh[k] = __floats2half2_rn(v[2 * k], v[2 * k + 1]);
+      // rotated K: k'[c] = cos*k[c] - sin*k[c+64] (c < 64), cos*k[c] + sin*k[c-64] (c >= 64); j = c mod 64
+      const uint4 o = dq_finish8<!IS_V && ROPE>(tile + gt * kTP, c0, cs + t * kRopePitch + (c0 & 63));
       __half* dst = p.out + (int64_t)(h0 + g) * p.head_stride + (t0 - p.start + t) * kHeadDim + c0;
       *reinterpret_cast<uint4*>(dst) = o;
     }
