@@ -213,7 +213,7 @@ def head_err(got, want):
 CONFIGS = [(4, 32, "kv", False, 0, 0), (3, 32, "kv", False, 5, 0), (2, 32, "kv", False, 0, 70_000),
            (4, 4, "kv", False, 5, 0), (4, 40, "dense", False, 0, 0), (4, 64, "k_only", False, 5, 65_530),
            (2, 32, "kv", True, 5, 0), (4, 32, "kv", True, 0, 0), (3, 40, "k_only", False, 0, 0),
-           (2, 64, "dense", False, 5, 0)]
+           (2, 64, "dense", False, 5, 0), (4, 4, "kv", False, 130, 0), (3, 32, "k_only", False, 64, 70_000)]
 # (T, L): every T edge of the query blocks and every L edge of the key tiles, and lengths where the split count
 # changes (at T = 1, 32 heads: 1, 1, 2, 3, 4 splits for L = 0, 64, 65, 129, 193)
 SHAPES = [(1, 1000), (15, 0), (16, 1), (17, 63), (BQ - 1, 64), (BQ, 65), (BQ + 1, 1000), (300, 1000), (2048, 1000),
