@@ -61,6 +61,13 @@ template <int BITS> struct KRCfg {
   static constexpr uint32_t kStage = (kKRWarps / kBoxWarps) * kBox;   // one slab = one head x 240 tokens
 };
 
+// tokens per CTA when L tokens are cut into at most `splits` ranges of whole 16-token warp columns: the finest rounding
+// the kernel allows, so that long caches give every SM a range (the last round's columns are spread over the warps)
+__host__ __device__ __forceinline__ int64_t kr_range(int64_t L, int64_t splits) {
+  const int64_t r = (L + splits - 1) / splits;
+  return (r + kKRColTok - 1) / kKRColTok * kKRColTok;
+}
+
 template <int IMM> __device__ __forceinline__ uint32_t kr_lds_word(uint32_t addr) {
   uint32_t v;
   asm volatile("ld.shared.u32 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(IMM));
@@ -215,8 +222,7 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
       const int64_t r = (L_eff + gridDim.x - 1) / gridDim.x;
       range = (r + kPageQuantum - 1) / kPageQuantum * kPageQuantum;
     } else {
-      const int64_t r = (L_eff + gridDim.x - 1) / gridDim.x;
-      range = (r + 31) & ~(int64_t)31;
+      range = kr_range(L_eff, gridDim.x);
     }
   }
   const int64_t t_begin = p.t0 + (int64_t)blockIdx.x * range;
@@ -279,28 +285,37 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
   hs.rot = hs.half ? 30u : 2u;
   hs.bias = hs.half * (BITS == 4 ? 0x40404040u : (BITS == 2 ? 0x10101010u : 0x20u));
   const uint32_t rat0 = smem_u32(s_rat) + hs.half * 32u;
-  const uint32_t stage0 = smem_u32(s_stage) + (uint32_t)(warp / C::kBoxWarps) * C::kBox +
-                          (uint32_t)((warp % C::kBoxWarps) * kKRColTok + tl) * 4u;
   mbar_wait(s_tabbar, 0);
   int s = 0;
   uint32_t ph = 0;
   for (int r = 0; r < nrounds; ++r) {
-    const int col = r * kKRWarps + warp;
-    const bool live = col < ncols;                       // warp-uniform
-    const int64_t t = t_begin + (int64_t)col * kKRColTok + tl;
-    const bool mine = live && t < t_limit;
+    // A round's slabs hold nlive columns (15; fewer in a CTA's last round).  Every column gets the warps w with
+    // w % nlive == c; the m of them split its heads round-robin (warp w takes heads w / nlive, + m, ...), so a short last
+    // round keeps all 15 warps busy on the slabs the ring holds at once, and a warp keeps one column (one cos/sin
+    // load) per round.  A full round is one column per warp for every head.
+    const int nlive = min(kKRWarps, ncols - r * kKRWarps);
+    const int c = warp % nlive;
+    const int64_t t = t_begin + (int64_t)(r * kKRWarps + c) * kKRColTok + tl;
+    const bool mine = t < t_limit;
     float2 cs[32];
-    if (live) {
+    if (warp / nlive < nh) {
       const float2* rp = p.rope + (mine ? (t + p.pos_offset) : 0) + (int64_t)hs.half * p.rope_npos;
 #pragma unroll
       for (int k = 0; k < 32; ++k)      // pair of register k: channel 8 (k/4) + 2 (k%4) + half
         cs[k] = mine ? ld_keep_f2(rp + (int64_t)(8 * (k >> 2) + 2 * (k & 3)) * p.rope_npos, pol_keep) : make_float2(0.f, 0.f);
     }
-    // GQA: the grp query heads of a KV head are consecutive; the first waits for the slab, the last releases it
+    const int m = (kKRWarps - 1 - c) / nlive + 1;
+    int next_h = warp / nlive;                           // this warp's next head (warp-uniform)
+    const uint32_t stage0 = smem_u32(s_stage) + (uint32_t)(c / C::kBoxWarps) * C::kBox +
+                            (uint32_t)((c % C::kBoxWarps) * kKRColTok + tl) * 4u;
+    // GQA: the grp query heads of a KV head are consecutive; the first waits for the slab, the last releases it.
+    // Every warp waits for and releases every slab, its heads or not, so the ring's arrive counts stay kKRWarps.
     for (int hl = 0; hl < nh; ++hl) {
+      const bool live = hl == next_h;                    // warp-uniform
+      if (live) next_h += m;
       float* optr = p.out + boff + (int64_t)(h0 + hl) * p.out_stride + t;
       float old = 0.f;
-      if (p.accumulate && mine && hs.half == 0) old = __ldcg(optr);
+      if (p.accumulate && live && mine && hs.half == 0) old = __ldcg(optr);
       if (!GQA || hl % grp == 0) mbar_wait(&s_full[s], ph);
       if (live) {
         float acc = k_ratio_head<BITS>(stage0 + (uint32_t)s * C::kStage, tab0 + (uint32_t)hl * C::kHeadTab,
@@ -420,7 +435,7 @@ static int launch_k_ratio(KRParams p, int grp, const float* q, const float* lut,
   const int sms = num_sms_cached();
   const int per = B > 0 ? groups * B : groups;   // a batch shares the SMs among its B x groups CTA columns
   const int64_t max_splits = sms / per > 0 ? sms / per : 1;
-  p.range = k_token_range(p.L, max_splits);
+  p.range = kr_range(p.L, max_splits);
   const int64_t splits = (p.L + p.range - 1) / p.range;
   if (pg != nullptr) {
     const dim3 grid((unsigned)splits, (unsigned)groups, (unsigned)B);
