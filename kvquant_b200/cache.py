@@ -286,52 +286,37 @@ class LayerCache:
         lets partial results over disjoint token ranges be merged exactly (sequence-sharded decode).
         Grouped-query cache: q, out f32 [q_heads, 128], lse [q_heads] (kvq_attend_gqa)."""
         if self.group > 1:
-            return self._attend_gqa(q, None, 0, rope_theta, out, lse, None)
-        L = self.len
-        if self.v_norm is not None and not self.use_native_v:
+            self._gqa_check()
+        elif self.v_norm is not None and not self.use_native_v:
             # the per-token LUT rows hold the un-normed centroids while the outlier residuals were taken against the
             # Q-Norm table: the legacy-LUT V kernel would mix the two
             raise NotImplementedError("V Q-Norm needs the native V form (use_native_v=True)")
-        self._ensure_scratch(self.lib.kvq_attend_scratch_bytes(self.H, max(L, 1)), 1.25)
-        pos_offset = self.n_sink + self.pos_base
-        rope, rope_h, npos = qc.rope_tables(self.device, rope_theta, L + pos_offset + 1)
-        fast = self.precision == "fp16" and self.use_native_v
-        out = self._out if out is None else out
-        ns = self.n_sink if self.sink_k is not None else 0
-        _lib.check(self.lib.kvq_attend(
-            self.bits, self._vec(q, self.hidden, "q"), self.kcache.data_ptr(), self.klut_deq.data_ptr(), *self._out_ptrs("k"),
-            self.vcache.data_ptr(), self.vlut.data_ptr(),
-            self.v_cent_deq.data_ptr() if self.use_native_v else None, self.vaff.data_ptr() if self.use_native_v else None,
-            *self._out_ptrs("v"),
-            self.n_out, self.H, self.Lmax, L, rope.data_ptr(), npos, float(rope_theta), pos_offset,
-            self.sink_k.data_ptr() if ns else None, self.sink_v.data_ptr() if ns else None, ns,
-            self._vec(out, self.hidden, "out"), self._vec(lse, self.H, "lse") if lse is not None else None, self._scratch.data_ptr(),
-            rope_h.data_ptr() if fast else None, torch.cuda.current_stream().cuda_stream), "kvq_attend")
-        return out
+        return self._attend(q, None, 0, rope_theta, out, lse, self.len)
 
-    def _attend_gqa(self, q, len_dev, len_add, rope_theta, out, lse, L_cap):
-        """attend (len_dev None) or attend_dyn of a grouped-query cache: kvq_attend_gqa[_dyn]."""
-        self._gqa_check()
-        L = self.len if len_dev is None else (self.Lmax if L_cap is None else int(L_cap))
+    def _attend(self, q, len_dev, len_add, rope_theta, out, lse, L):
+        """attend over L slots (len_dev None: kvq_attend_gqa) or attend_dyn with the cap L (kvq_attend_gqa_dyn).  With
+        one KV head per query head the C entry points are kvq_attend / kvq_attend_dyn themselves."""
+        native, mha = self.use_native_v, self.group == 1
         self._ensure_scratch(self.lib.kvq_attend_scratch_bytes(self.Hq, max(L, 1)), 1.25 if len_dev is None else 1.0)
         pos_offset = self.n_sink + self.pos_base
-        rope, _, npos = qc.rope_tables(self.device, rope_theta, L + pos_offset + 1)
+        rope, rope_h, npos = qc.rope_tables(self.device, rope_theta, L + pos_offset + 1)
+        fast = self.precision == "fp16" and native and mha
         out = self._out if out is None else out
         ns = self.n_sink if self.sink_k is not None else 0
-        kpart = (self.kcache.data_ptr(), self.klut_deq.data_ptr(), *self._out_ptrs("k"), self.vcache.data_ptr())
-        vpart = (self.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._out_ptrs("v"), self.n_out, self.Hq, self.H,
-                 self.Lmax, L)
+        head = (self.bits, self._vec(q, self.q_hidden, "q"), self.kcache.data_ptr(), self.klut_deq.data_ptr(),
+                *self._out_ptrs("k"), self.vcache.data_ptr())
+        vpart = (self.v_cent_deq.data_ptr() if native else None, self.vaff.data_ptr() if native else None,
+                 *self._out_ptrs("v"), self.n_out, self.Hq, self.H, self.Lmax, L)
         tail = (rope.data_ptr(), npos, float(rope_theta), pos_offset, self.sink_k.data_ptr() if ns else None,
                 self.sink_v.data_ptr() if ns else None, ns, self._vec(out, self.q_hidden, "out"),
-                self._vec(lse, self.Hq, "lse") if lse is not None else None, self._scratch.data_ptr(), None,
-                torch.cuda.current_stream().cuda_stream)
-        qp = self._vec(q, self.q_hidden, "q")
+                self._vec(lse, self.Hq, "lse") if lse is not None else None, self._scratch.data_ptr(),
+                rope_h.data_ptr() if fast else None, torch.cuda.current_stream().cuda_stream)
         if len_dev is None:
-            _lib.check(self.lib.kvq_attend_gqa(self.bits, qp, *kpart, None, *vpart, *tail), "kvq_attend_gqa")
+            vlut = self.vlut.data_ptr() if mha else None
+            _lib.check(self.lib.kvq_attend_gqa(*head, vlut, *vpart, *tail), "kvq_attend_gqa")
         else:
-            _lib.check(self.lib.kvq_attend_gqa_dyn(self.bits, qp, *kpart, *vpart,
-                                                   self._vec(len_dev, 1, "len_dev", torch.int64), int(len_add), *tail),
-                       "kvq_attend_gqa_dyn")
+            _lib.check(self.lib.kvq_attend_gqa_dyn(*head, *vpart, self._vec(len_dev, 1, "len_dev", torch.int64),
+                                                   int(len_add), *tail), "kvq_attend_gqa_dyn")
         return out
 
     # -- device-resident length (one captured CUDA graph serves a growing cache; SURVEY.md 8(f)-2) ----------------------
@@ -353,25 +338,10 @@ class LayerCache:
         """attend() over `min(len_dev[0] + len_add, L_cap)` slots, the length read on the device; grids, scratch and
         the rope table are sized for L_cap (default: the whole allocation)."""
         if self.group > 1:
-            return self._attend_gqa(q, len_dev, len_add, rope_theta, out, lse, L_cap)
-        if not self.use_native_v:
+            self._gqa_check()
+        elif not self.use_native_v:
             raise NotImplementedError("device-resident length needs the native V form")
-        L_cap = self.Lmax if L_cap is None else int(L_cap)
-        self._ensure_scratch(self.lib.kvq_attend_scratch_bytes(self.H, max(L_cap, 1)), 1.0)
-        pos_offset = self.n_sink + self.pos_base
-        rope, rope_h, npos = qc.rope_tables(self.device, rope_theta, L_cap + pos_offset + 1)
-        fast = self.precision == "fp16"
-        out = self._out if out is None else out
-        ns = self.n_sink if self.sink_k is not None else 0
-        _lib.check(self.lib.kvq_attend_dyn(
-            self.bits, self._vec(q, self.hidden, "q"), self.kcache.data_ptr(), self.klut_deq.data_ptr(), *self._out_ptrs("k"),
-            self.vcache.data_ptr(), self.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._out_ptrs("v"),
-            self.n_out, self.H, self.Lmax, L_cap, self._vec(len_dev, 1, "len_dev", torch.int64), int(len_add), rope.data_ptr(), npos,
-            float(rope_theta), pos_offset, self.sink_k.data_ptr() if ns else None,
-            self.sink_v.data_ptr() if ns else None, ns, self._vec(out, self.hidden, "out"),
-            self._vec(lse, self.H, "lse") if lse is not None else None, self._scratch.data_ptr(),
-            rope_h.data_ptr() if fast else None, torch.cuda.current_stream().cuda_stream), "kvq_attend_dyn")
-        return out
+        return self._attend(q, len_dev, len_add, rope_theta, out, lse, self.Lmax if L_cap is None else int(L_cap))
 
     def _kv_out(self, t, n, name):
         """Caller-supplied fp16 [H, n, 128] output, possibly a view into a larger [H, S, 128] buffer: tokens and

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cuda.h>
 #include <stdint.h>
+#include <type_traits>
 #include "../../include/kvquant_b200.h"
 
 #ifndef __CUDA_ARCH__
@@ -204,8 +205,20 @@ __device__ __forceinline__ int page_of(const PageRef& pg, int b, int t) {
   return pg.table[b * pg.max_pages + t / pg.P];
 }
 
-// host: build a 2D tensor map over the packed cache viewed as uint32 [rows = H*W, cols = Lmax]
+// host: build a 2D tensor map over the packed cache viewed as uint32 [rows = H*W, cols = Lmax]  (kvq_capi.cu)
 int make_cache_tensor_map(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                           uint32_t box_cols, uint32_t box_rows, int swizzle_bytes);
+// host: SM count of the current device, queried once per device  (kvq_capi.cu)
+int num_sms_cached();
+
+// host: the kernel flavour of a call as compile-time constants.  Calls f(GQA, BATCH, PAGED) with std::bool_constant
+// arguments (GQA() is a constant expression, usable as a template argument) for exactly the six flavours that exist: a
+// paged call is a batch, so there is no <BATCH = false, PAGED = true> instantiation.
+template <class F>
+inline auto with_flavour(bool gqa, bool batch, bool paged, F&& f) {
+  auto g = [&](auto b, auto p) { return gqa ? f(std::true_type{}, b, p) : f(std::false_type{}, b, p); };
+  return paged ? g(std::true_type{}, std::true_type{})
+       : batch ? g(std::true_type{}, std::false_type{}) : g(std::false_type{}, std::false_type{});
+}
 
 }  // namespace kvq

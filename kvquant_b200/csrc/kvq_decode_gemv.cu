@@ -123,8 +123,6 @@ __global__ void __launch_bounds__(kGemvThreads, 1) dec_gemv_kernel(
   }
 }
 
-int num_sms_cached();
-
 }  // namespace kvq
 
 using namespace kvq;

@@ -23,6 +23,7 @@
 //     apart by up to a ring.
 // Per element: 1 PRMT (3-bit: SHF+LOP3) + 1 LDS.32 + 2 half->float conversions + 2 FFMA.
 #include "kvq_kscore.cuh"
+#include "kvq_attend.cuh"
 #include <cuda_fp16.h>
 
 namespace kvq {
@@ -366,8 +367,6 @@ __global__ void rope_table_half_kernel(uint32_t* __restrict__ out, float rope_th
   }
 }
 
-int num_sms_cached();
-
 template <int BITS>
 static int launch_k_fast(KFParams p, const float* q, const float* lut, uint32_t* qtab, const int32_t* cache, int run_prep,
                          cudaStream_t st) {
@@ -404,23 +403,21 @@ static int launch_k_fast(KFParams p, const float* q, const float* lut, uint32_t*
   return 0;
 }
 
-// dense K scores of the fused attend, fp16-table form.  `scores` holds the (unscaled) outlier partial sums on entry
-// when accumulate != 0.
-int k_fast_dispatch(int bits, const float* q, const int32_t* cache, float* scores, int64_t score_stride, const float* lut,
-                    int H, int64_t Lmax, int64_t L, const void* rope_half, int64_t rope_npos, int pos_offset, float* gmax,
-                    float scale, int accumulate, const int64_t* len_dev, int64_t len_add, void* qtab, int64_t t0,
-                     int run_prep, cudaStream_t st) {
+// dense K scores of the fused attend, fp16-table form, tokens [t0, t0 + Lb).  s.scores holds the (unscaled) outlier
+// partial sums on entry when accumulate != 0.
+int k_fast_dispatch(const AttendCall& c, const AttendScratch& s, int64_t t0, int64_t Lb, int run_prep, int accumulate) {
   KFParams p{};
-  p.qtab = static_cast<const uint32_t*>(qtab);
-  p.rope_h = static_cast<const uint32_t*>(rope_half);
-  p.out = scores; p.gmax = gmax;
-  p.Lmax = Lmax; p.L = L; p.out_stride = score_stride; p.rope_npos = rope_npos;
-  p.len_dev = len_dev; p.len_add = len_add; p.t0 = t0;
-  p.H = H; p.pos_offset = pos_offset; p.accumulate = accumulate; p.scale = scale;
-  switch (bits) {
-    case 4: return launch_k_fast<4>(p, q, lut, static_cast<uint32_t*>(qtab), cache, run_prep, st);
-    case 3: return launch_k_fast<3>(p, q, lut, static_cast<uint32_t*>(qtab), cache, run_prep, st);
-    case 2: return launch_k_fast<2>(p, q, lut, static_cast<uint32_t*>(qtab), cache, run_prep, st);
+  uint32_t* qtab = reinterpret_cast<uint32_t*>(s.qtab);
+  p.qtab = qtab;
+  p.rope_h = static_cast<const uint32_t*>(c.rope_half);
+  p.out = s.scores; p.gmax = s.gmax;
+  p.Lmax = c.Lmax; p.L = Lb; p.out_stride = s.stride; p.rope_npos = c.rope_npos;
+  p.len_dev = c.len_dev; p.len_add = c.len_add; p.t0 = t0;
+  p.H = c.Hq; p.pos_offset = c.pos_offset; p.accumulate = accumulate; p.scale = kAttendScale;
+  switch (c.bits) {
+    case 4: return launch_k_fast<4>(p, c.q, c.klut, qtab, c.kcache, run_prep, c.stream);
+    case 3: return launch_k_fast<3>(p, c.q, c.klut, qtab, c.kcache, run_prep, c.stream);
+    case 2: return launch_k_fast<2>(p, c.q, c.klut, qtab, c.kcache, run_prep, c.stream);
     default: return KVQ_E_BITS;
   }
 }

@@ -26,6 +26,7 @@
 // cut the register budget from 128 to 96 (a lane holds 64 registers of cos/sin), and a TMA issue rotating over the
 // consumer warps measured 40 % slower (the issuing warp waits for the slowest warp before it may start its own slab).
 #include "kvq_kscore.cuh"
+#include "kvq_attend.cuh"
 
 namespace kvq {
 
@@ -375,9 +376,7 @@ __global__ void k_ratio_prep_kernel(const float* __restrict__ q, const float* __
   qrat[(int64_t)h * kHeadDim + gi * 16 + half * 8 + xy * 4 + k] = sg * qb / qa;
 }
 
-int num_sms_cached();
-
-template <int BITS, bool GQA, bool BATCH, bool PAGED = false>
+template <int BITS, bool GQA, bool BATCH, bool PAGED>
 static int set_k_ratio_smem() {
   static PerDeviceOnce attr_once;
   bool& attr_done = attr_once.cur();
@@ -389,22 +388,19 @@ static int set_k_ratio_smem() {
   return 0;
 }
 
-// B == 0: one sequence; B >= 1: a batch of B sequences, each with its own scratch block of bstride floats;
-// pg != nullptr: a paged batch (the grid is the contiguous batch's)
+// c.B == 0: one sequence; c.B >= 1: a batch of B sequences, each with its own scratch block of s.bstride floats;
+// c.pg != nullptr: a paged batch (the grid is the contiguous batch's)
 template <int BITS>
-static int launch_k_ratio(KRParams p, int grp, const float* q, const float* lut, float* qtab, float* qrat,
-                          const int32_t* cache, int run_prep, cudaStream_t st, int B = 0, int64_t bstride = 0,
-                          const PageRef* pg = nullptr) {
+static int launch_k_ratio(KRParams p, const AttendCall& c, const AttendScratch& s, int run_prep) {
   using C = KRCfg<BITS>;
-  const bool gqa = grp > 1;
+  const int B = c.B, grp = c.grp();
+  const bool gqa = grp > 1, batch = B > 0, paged = c.pg != nullptr;
+  cudaStream_t st = c.stream;
   if (run_prep) {
-    if (B > 0) {
-      if (gqa) k_ratio_prep_kernel<BITS, true, true><<<dim3(p.H, B), kHeadDim, 0, st>>>(q, lut, qtab, qrat, grp, bstride);
-      else k_ratio_prep_kernel<BITS, false, true><<<dim3(p.H, B), kHeadDim, 0, st>>>(q, lut, qtab, qrat, 1, bstride);
-    } else {
-      if (gqa) k_ratio_prep_kernel<BITS, true, false><<<p.H, kHeadDim, 0, st>>>(q, lut, qtab, qrat, grp, 0);
-      else k_ratio_prep_kernel<BITS, false, false><<<p.H, kHeadDim, 0, st>>>(q, lut, qtab, qrat, 1, 0);
-    }
+    with_flavour(gqa, batch, false, [&](auto GQA, auto BATCH, auto) {
+      k_ratio_prep_kernel<BITS, GQA(), BATCH()><<<batch ? dim3(p.H, B) : dim3(p.H), kHeadDim, 0, st>>>(
+          c.q, c.klut, s.qtab, s.qrat, grp, s.bstride);
+    });
     KVQ_LAUNCH_CHECK();
   }
   // CTA head groups of at most GMAX query heads; under GQA whole KV-head groups (grp <= 16 <= GMAX)
@@ -418,61 +414,48 @@ static int launch_k_ratio(KRParams p, int grp, const float* q, const float* lut,
   if (S < 2) return KVQ_E_UNSUPPORTED;
   p.n_stages = S;
   const size_t smem = (size_t)tab_span + (size_t)S * C::kStage + 8u * (2 * S + 1) + 4u * p.G + 1024u;
-  int rc = pg != nullptr ? (gqa ? set_k_ratio_smem<BITS, true, true, true>() : set_k_ratio_smem<BITS, false, true, true>())
-         : B > 0 ? (gqa ? set_k_ratio_smem<BITS, true, true>() : set_k_ratio_smem<BITS, false, true>())
-                 : (gqa ? set_k_ratio_smem<BITS, true, false>() : set_k_ratio_smem<BITS, false, false>());
+  int rc = with_flavour(gqa, batch, paged, [](auto GQA, auto BATCH, auto PAGED) {
+    return set_k_ratio_smem<BITS, GQA(), BATCH(), PAGED()>();
+  });
   if (rc != 0) return rc;
   CUtensorMap tmap;
   // a batch: one map over the B sequences' caches, B*Hkv*W rows (sequence b's rows follow b*Hkv*W others);
   // a paged batch: one map over the pool, n_pool*Hkv*W rows of P tokens
-  if (pg != nullptr)
-    rc = make_cache_tensor_map(&tmap, cache, (uint64_t)pg->n_pool * Hkv * C::W, (uint64_t)pg->P,
+  if (paged)
+    rc = make_cache_tensor_map(&tmap, c.kcache, (uint64_t)c.pg->n_pool * Hkv * C::W, (uint64_t)c.pg->P,
                                kKRColTok * C::kBoxWarps, C::W, /*swizzle*/ 0);
   else
-    rc = make_cache_tensor_map(&tmap, cache, (uint64_t)(B > 0 ? B : 1) * Hkv * C::W, (uint64_t)p.Lmax,
+    rc = make_cache_tensor_map(&tmap, c.kcache, (uint64_t)(batch ? B : 1) * Hkv * C::W, (uint64_t)p.Lmax,
                                kKRColTok * C::kBoxWarps, C::W, /*swizzle*/ 0);
   if (rc != 0) return rc;
   const int sms = num_sms_cached();
-  const int per = B > 0 ? groups * B : groups;   // a batch shares the SMs among its B x groups CTA columns
+  const int per = batch ? groups * B : groups;   // a batch shares the SMs among its B x groups CTA columns
   const int64_t max_splits = sms / per > 0 ? sms / per : 1;
   p.range = kr_range(p.L, max_splits);
   const int64_t splits = (p.L + p.range - 1) / p.range;
-  if (pg != nullptr) {
-    const dim3 grid((unsigned)splits, (unsigned)groups, (unsigned)B);
-    if (gqa) k_ratio_kernel<BITS, true, true, true><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, bstride, *pg);
-    else k_ratio_kernel<BITS, false, true, true><<<grid, kKRThreads, smem, st>>>(tmap, p, 1, bstride, *pg);
-  } else if (B > 0) {
-    const dim3 grid((unsigned)splits, (unsigned)groups, (unsigned)B);
-    if (gqa) k_ratio_kernel<BITS, true, true><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, bstride, PageRef{});
-    else k_ratio_kernel<BITS, false, true><<<grid, kKRThreads, smem, st>>>(tmap, p, 1, bstride, PageRef{});
-  } else {
-    const dim3 grid((unsigned)splits, (unsigned)groups);
-    if (gqa) k_ratio_kernel<BITS, true, false><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, 0, PageRef{});
-    else k_ratio_kernel<BITS, false, false><<<grid, kKRThreads, smem, st>>>(tmap, p, 1, 0, PageRef{});
-  }
+  const dim3 grid = batch ? dim3((unsigned)splits, (unsigned)groups, (unsigned)B) : dim3((unsigned)splits, (unsigned)groups);
+  with_flavour(gqa, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
+    k_ratio_kernel<BITS, GQA(), BATCH(), PAGED()><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, s.bstride,
+                                                                                  paged ? *c.pg : PageRef{});
+  });
   KVQ_LAUNCH_CHECK();
   return 0;
 }
 
-// dense K scores of the fused attend, fp32 ratio form.  `scores` holds the (unscaled) outlier partial sums on entry
-// when accumulate != 0.  qtab: scratch of H * 128 * (2^bits + 1) floats.  H query heads, grp of them per KV head.
-int k_ratio_dispatch(int bits, const float* q, const int32_t* cache, float* scores, int64_t score_stride, const float* lut,
-                     int H, int grp, int64_t Lmax, int64_t L, const float* rope, int64_t rope_npos, int pos_offset,
-                     float* gmax, float scale, int accumulate, const int64_t* len_dev, int64_t len_add, void* qtab,
-                     int64_t t0, int run_prep, cudaStream_t st, int B, int64_t bstride, const PageRef* pg) {
+// dense K scores of the fused attend, fp32 ratio form, tokens [t0, t0 + Lb).  s.scores holds the (unscaled) outlier
+// partial sums on entry when accumulate != 0.  s.qtab / s.qrat: Hq * 128 * (2^bits + 1) floats of scratch.
+int k_ratio_dispatch(const AttendCall& c, const AttendScratch& s, int64_t t0, int64_t Lb, int run_prep, int accumulate) {
   KRParams p{};
-  float* tab = static_cast<float*>(qtab);
-  float* rat = tab + (size_t)H * kHeadDim * (1 << bits);
-  p.qtab = tab; p.qrat = rat;
-  p.rope = reinterpret_cast<const float2*>(rope);
-  p.out = scores; p.gmax = gmax;
-  p.Lmax = Lmax; p.L = L; p.out_stride = score_stride; p.rope_npos = rope_npos;
-  p.len_dev = len_dev; p.len_add = len_add; p.t0 = t0;
-  p.H = H; p.pos_offset = pos_offset; p.accumulate = accumulate; p.scale = scale;
-  switch (bits) {
-    case 4: return launch_k_ratio<4>(p, grp, q, lut, tab, rat, cache, run_prep, st, B, bstride, pg);
-    case 3: return launch_k_ratio<3>(p, grp, q, lut, tab, rat, cache, run_prep, st, B, bstride, pg);
-    case 2: return launch_k_ratio<2>(p, grp, q, lut, tab, rat, cache, run_prep, st, B, bstride, pg);
+  p.qtab = s.qtab; p.qrat = s.qrat;
+  p.rope = reinterpret_cast<const float2*>(c.rope);
+  p.out = s.scores; p.gmax = s.gmax;
+  p.Lmax = c.Lmax; p.L = Lb; p.out_stride = s.stride; p.rope_npos = c.rope_npos;
+  p.len_dev = c.len_dev; p.len_add = c.len_add; p.t0 = t0;
+  p.H = c.Hq; p.pos_offset = c.pos_offset; p.accumulate = accumulate; p.scale = kAttendScale;
+  switch (c.bits) {
+    case 4: return launch_k_ratio<4>(p, c, s, run_prep);
+    case 3: return launch_k_ratio<3>(p, c, s, run_prep);
+    case 2: return launch_k_ratio<2>(p, c, s, run_prep);
     default: return KVQ_E_BITS;
   }
 }

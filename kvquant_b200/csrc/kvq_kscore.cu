@@ -20,6 +20,7 @@
 //   * per element: 1 address op (PRMT), 1 LDS.64, 2 FFMA; words and rope values are prefetched into rotating
 //     register buffers; token ranges are cut at warp granularity so that every SM gets an equal share.
 #include "kvq_kscore.cuh"
+#include "kvq_attend.cuh"
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include <algorithm>
@@ -486,9 +487,7 @@ static int launch_k_kappa(const KParams& p, cudaStream_t st) {
   if (rc != 0) return rc;
   const int n_groups = (p.H + C::G - 1) / C::G;
   const int64_t n_tiles = (p.L + C::TT - 1) / C::TT;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms_cached();
   const int64_t max_splits = sms / n_groups > 0 ? sms / n_groups : 1;
   KParams q = p;
   q.tiles_per_cta = (int)((n_tiles + max_splits - 1) / max_splits);
@@ -692,27 +691,32 @@ static bool k_out_direct(int64_t n_positions) {
   return n_positions > thr;
 }
 
-// zero_first = 1: `out` is a fresh score buffer (fused path) and is cleared before the scatter
-static int set_k_outlier_smem(size_t smem, bool gqa, bool batch = false, bool paged = false) {
+static int set_k_outlier_smem(size_t smem, bool gqa, bool batch, bool paged) {
   static size_t smem_set_dev[6][64];   // per kernel and device: largest dynamic shared memory opted in so far (0 = 48 KiB)
   int dev_idx = 0;
   cudaGetDevice(&dev_idx);
   size_t& smem_set = smem_set_dev[gqa + 2 * (batch + paged)][dev_idx & 63];
   if (smem_set == 0) smem_set = 48 * 1024;
   if (smem > smem_set) {
-    const int a = cudaFuncAttributeMaxDynamicSharedMemorySize;
-    cudaError_t e = paged ? (gqa ? cudaFuncSetAttribute(k_outlier_pers_kernel<true, true, true>, (cudaFuncAttribute)a, (int)smem)
-                                 : cudaFuncSetAttribute(k_outlier_pers_kernel<false, true, true>, (cudaFuncAttribute)a, (int)smem))
-                  : batch ? (gqa ? cudaFuncSetAttribute(k_outlier_pers_kernel<true, true>, (cudaFuncAttribute)a, (int)smem)
-                                 : cudaFuncSetAttribute(k_outlier_pers_kernel<false, true>, (cudaFuncAttribute)a, (int)smem))
-                          : (gqa ? cudaFuncSetAttribute(k_outlier_pers_kernel<true, false>, (cudaFuncAttribute)a, (int)smem)
-                                 : cudaFuncSetAttribute(k_outlier_pers_kernel<false, false>, (cudaFuncAttribute)a, (int)smem));
+    const cudaError_t e = with_flavour(gqa, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
+      return cudaFuncSetAttribute(k_outlier_pers_kernel<GQA(), BATCH(), PAGED()>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    });
     if (e != cudaSuccess) return (int)e;
     smem_set = smem;
   }
   return 0;
 }
 
+// persistent outlier CTAs along x for `total` entries per sequence: a few per SM (fewer when the q table is large),
+// that allowance shared among the nseq sequences of a batch
+static unsigned k_outlier_grid(int64_t total, size_t smem, int nseq) {
+  const int64_t want = (total + kOutPersThreads - 1) / kOutPersThreads;
+  const int per_sm = smem > 56 * 1024 ? 2 : 4;
+  const int64_t cap = std::max<int64_t>(1, (int64_t)num_sms_cached() * per_sm / nseq);
+  return (unsigned)std::max<int64_t>(1, std::min(want, cap));
+}
+
+// zero_first = 1: `out` is a fresh score buffer (fused path) and is cleared before the scatter
 // p.H counts query heads, p.grp of them per KV head (the entries' channels are KV channels)
 static int launch_k_outliers(const KParams& p, int zero_first, float scale, cudaStream_t st) {
   const bool gqa = p.grp > 1;
@@ -732,29 +736,19 @@ static int launch_k_outliers(const KParams& p, int zero_first, float scale, cuda
     KVQ_LAUNCH_CHECK();
     return 0;
   }
-  const int rc = set_k_outlier_smem(smem, gqa);
+  const int rc = set_k_outlier_smem(smem, gqa, false, false);
   if (rc != 0) return rc;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int64_t want = (total + kOutPersThreads - 1) / kOutPersThreads;
-  const int per_sm = smem > 56 * 1024 ? 2 : 4;
-  const unsigned grid = (unsigned)(want < (int64_t)sms * per_sm ? want : (int64_t)sms * per_sm);
+  const unsigned grid = k_outlier_grid(total, smem, 1);
   // token-major target (fused path): a token's heads share one 128-byte line, so a warp's ~25 reductions (one or
   // two tokens) coalesce into one or two L1 requests instead of one per head row
   float* dst = p.opart != nullptr ? const_cast<float*>(p.opart) : p.out;
   const int64_t sh = p.opart != nullptr ? 1 : p.out_stride, stt = p.opart != nullptr ? p.opart_stride : 1;
   const float direct_theta = k_out_direct(p.L + p.pos_offset) ? p.theta : 0.f;
-  if (gqa)
-    k_outlier_pers_kernel<true, false><<<grid, kOutPersThreads, smem, st>>>(p.q, p.outliers, p.outlier_idx, dst, sh, stt, p.L,
-                                                                     p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset,
-                                                                     scale, p.len_dev, p.len_add, p.rope_h, direct_theta,
-                                                                     p.grp, 0, 0, PageRef{});
-  else
-    k_outlier_pers_kernel<false, false><<<grid, kOutPersThreads, smem, st>>>(p.q, p.outliers, p.outlier_idx, dst, sh, stt, p.L,
-                                                                      p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset,
-                                                                      scale, p.len_dev, p.len_add, p.rope_h, direct_theta,
-                                                                      1, 0, 0, PageRef{});
+  with_flavour(gqa, false, false, [&](auto GQA, auto BATCH, auto PAGED) {
+    k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem, st>>>(
+        p.q, p.outliers, p.outlier_idx, dst, sh, stt, p.L, p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset, scale,
+        p.len_dev, p.len_add, p.rope_h, direct_theta, gqa ? p.grp : 1, 0, 0, PageRef{});
+  });
   KVQ_LAUNCH_CHECK();
   return 0;
 }
@@ -787,9 +781,7 @@ static int launch_k_scores(const KParams& p, cudaStream_t st) {
     attr_done = true;
   }
   const int n_groups = (p.H + C::G - 1) / C::G;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms_cached();
   const int64_t max_splits = sms / n_groups > 0 ? sms / n_groups : 1;
   KParams q = p;
   q.range = k_token_range(p.L, max_splits);
@@ -833,38 +825,38 @@ int k_scores_dispatch(int bits, const KParams& p, cudaStream_t st) {
   }
 }
 
-int k_scores_fused(int bits, const float* q, const int32_t* cache, float* scores, int64_t score_stride,
-                   const float* lut, const float* outliers, const int32_t* outlier_idx, int n_out, int H,
-                   int64_t Lmax, int64_t L, const float* rope, int64_t rope_npos, float theta, int pos_offset,
-                   float* gmax, float scale, const int64_t* len_dev, int64_t len_add, float* opart, int opart_stride,
-                   cudaStream_t st) {
+// the KParams of a single-sequence fused attend, before the per-pass fields
+static KParams k_fused_params(const AttendCall& c, const AttendScratch& s) {
   KParams p{};
-  p.len_dev = len_dev; p.len_add = len_add;
-  p.q = q; p.cache = reinterpret_cast<const uint32_t*>(cache); p.out = scores; p.lut = lut;
-  p.outliers = outliers; p.outlier_idx = outlier_idx; p.rope = reinterpret_cast<const float2*>(rope);
-  p.gmax = gmax; p.Lmax = Lmax; p.L = L; p.out_stride = score_stride; p.rope_npos = rope_npos;
-  p.H = H; p.n_out = n_out; p.pos_offset = pos_offset; p.scale = scale; p.accumulate = 0; p.theta = theta;
-  if (outliers != nullptr) {
+  p.len_dev = c.len_dev; p.len_add = c.len_add;
+  p.q = c.q; p.out = s.scores; p.rope = reinterpret_cast<const float2*>(c.rope);
+  p.Lmax = c.Lmax; p.L = c.L; p.out_stride = s.stride; p.rope_npos = c.rope_npos;
+  p.H = c.Hq; p.n_out = c.n_out; p.pos_offset = c.pos_offset; p.theta = c.theta;
+  return p;
+}
+
+int k_scores_fused(const AttendCall& c, const AttendScratch& s) {
+  KParams p = k_fused_params(c, s);
+  p.cache = reinterpret_cast<const uint32_t*>(c.kcache); p.lut = c.klut;
+  p.outliers = c.k_outliers; p.outlier_idx = c.k_outlier_idx;
+  p.gmax = s.gmax; p.scale = kAttendScale; p.accumulate = 0;
+  if (c.k_outliers != nullptr) {
     // outlier contributions are deposited UNSCALED (the dense kernel applies `scale` to partial + S), token-major
-    // when the caller provides the partial buffer (and the variant in use supports it)
-    const bool tm = opart != nullptr && !k_out_impl_table() && k_impl() == 0;
-    if (tm) { p.opart = opart; p.opart_stride = opart_stride; }
-    const int rc = launch_k_outliers(p, /*zero_first=*/1, 1.f, st);
+    // when the variant in use supports it
+    const bool tm = !k_out_impl_table() && k_impl() == 0;
+    if (tm) { p.opart = s.opart; p.opart_stride = s.opart_stride; }
+    const int rc = launch_k_outliers(p, /*zero_first=*/1, 1.f, c.stream);
     if (rc != 0) return rc;
     if (!tm) p.accumulate = 1;
   }
-  return k_scores_dispatch(bits, p, st);
+  return k_scores_dispatch(c.bits, p, c.stream);
 }
 
 // K side of the fused attend: outlier scatter straight into the head-major score buffer (cleared first), then the
 // TMA-fed dense kernel folds it in: out = (partial + S) * scale.  rope_half == null: exact fp32 ratio form
 // (kvq_kratio.cu); otherwise the fp16-table form (kvq_kfast.cu).
-// GQA: H query heads, grp per KV head (exact ratio form only: rope_half must be null when grp > 1)
-int k_scores_fused_fast(int bits, const float* q, const int32_t* cache, float* scores, int64_t score_stride,
-                        const float* lut, const float* outliers, const int32_t* outlier_idx, int n_out, int H, int grp,
-                        int64_t Lmax, int64_t L, const float* rope, const void* rope_half, int64_t rope_npos, float theta,
-                        int pos_offset, float* gmax, float scale, const int64_t* len_dev, int64_t len_add, void* qtab,
-                        cudaStream_t st) {
+// GQA: Hq query heads, grp per KV head (exact ratio form only: rope_half must be null when grp > 1)
+int k_scores_fused_fast(const AttendCall& c, const AttendScratch& s) {
   // KVQ_K_BLOCK=<tokens>: walk the cache in blocks whose score rows (H x block floats) stay L2-resident between the
   // outlier scatter (atomic adds) and the dense kernel.  The default is ONE pass; the switch stays for A/B runs and is
   // covered by tests/test_gpu_variants.py.
@@ -875,27 +867,22 @@ int k_scores_fused_fast(int bits, const float* q, const int32_t* cache, float* s
     if (kBlock < 32) kBlock = (int64_t)1 << 40;
   }
   int run_prep = 1;
-  for (int64_t t0 = 0; t0 < L; t0 += kBlock) {
-    const int64_t Lb = (L - t0 > kBlock + kBlock / 2) ? kBlock : (L - t0);   // the last block may be up to 1.5 blocks
+  for (int64_t t0 = 0; t0 < c.L; t0 += kBlock) {
+    const int64_t Lb = (c.L - t0 > kBlock + kBlock / 2) ? kBlock : (c.L - t0);   // the last block may be up to 1.5 blocks
     int accumulate = 0;
-    if (outliers != nullptr) {
-      KParams p{};
-      p.len_dev = len_dev; p.len_add = len_add - t0;
-      p.q = q; p.out = scores + t0; p.outliers = outliers + t0 * n_out; p.outlier_idx = outlier_idx + t0 * n_out;
-      p.rope = reinterpret_cast<const float2*>(rope); p.rope_h = static_cast<const uint32_t*>(rope_half);
-      p.Lmax = Lmax; p.L = Lb; p.out_stride = score_stride; p.rope_npos = rope_npos;
-      p.H = H; p.n_out = n_out; p.pos_offset = pos_offset + (int)t0; p.theta = theta; p.grp = grp;
-      cudaError_t e = cudaMemset2DAsync(scores + t0, sizeof(float) * (size_t)score_stride, 0, sizeof(float) * (size_t)Lb, (size_t)H, st);
+    if (c.k_outliers != nullptr) {
+      KParams p = k_fused_params(c, s);
+      p.len_add = c.len_add - t0; p.out = s.scores + t0; p.L = Lb; p.pos_offset = c.pos_offset + (int)t0;
+      p.outliers = c.k_outliers + t0 * c.n_out; p.outlier_idx = c.k_outlier_idx + t0 * c.n_out;
+      p.rope_h = static_cast<const uint32_t*>(c.rope_half); p.grp = c.grp();
+      cudaError_t e = cudaMemset2DAsync(s.scores + t0, sizeof(float) * (size_t)s.stride, 0, sizeof(float) * (size_t)Lb, (size_t)c.Hq, c.stream);
       if (e != cudaSuccess) return (int)e;
-      const int rc = launch_k_outliers(p, /*zero_first=*/0, 1.f, st);
+      const int rc = launch_k_outliers(p, /*zero_first=*/0, 1.f, c.stream);
       if (rc != 0) return rc;
       accumulate = 1;
     }
-    const int rc = (rope_half == nullptr)     // exact mode: fp32 ratio form (kvq_kratio.cu); else the fp16-table form
-        ? k_ratio_dispatch(bits, q, cache, scores, score_stride, lut, H, grp, Lmax, Lb, rope, rope_npos, pos_offset, gmax, scale,
-                           accumulate, len_dev, len_add, qtab, t0, run_prep, st)
-        : k_fast_dispatch(bits, q, cache, scores, score_stride, lut, H, Lmax, Lb, rope_half, rope_npos, pos_offset, gmax,
-                          scale, accumulate, len_dev, len_add, qtab, t0, run_prep, st);
+    const int rc = (c.rope_half == nullptr) ? k_ratio_dispatch(c, s, t0, Lb, run_prep, accumulate)
+                                            : k_fast_dispatch(c, s, t0, Lb, run_prep, accumulate);
     if (rc != 0) return rc;
     run_prep = 0;
     if (Lb != kBlock) break;
@@ -914,57 +901,35 @@ __global__ void k_batch_zero_kernel(float* __restrict__ scores, int64_t stride, 
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < L; t += (int64_t)gridDim.x * blockDim.x) row[t] = 0.f;
 }
 
-int num_sms_cached();
-
 // K side of the batched attend (kvq_attend_batch): exact fp32 ratio form, one launch per kernel for all B sequences.
 // q [B][H][128]; cache [B][Hkv*W][Lmax]; outlier rows [B][Lmax][n_out]; scores, gmax and qtab of sequence b at
-// b * bstride floats (sequence b's scratch block); the grids are sized for L_cap, each CTA reads its own length.
-// pg != nullptr: the paged batch (kvq_attend_paged), cache and outlier rows page pools; the score clear works on
+// b * bstride floats (sequence b's scratch block); the grids are sized for the cap c.L, each CTA reads its own length.
+// c.pg != nullptr: the paged batch (kvq_attend_paged), cache and outlier rows page pools; the score clear works on
 // logical token indices in the scratch and is the same.
-int k_scores_batch(int bits, int B, const float* q, const int32_t* cache, float* scores, int64_t score_stride,
-                   const float* lut, const float* outliers, const int32_t* outlier_idx, int n_out, int H, int grp,
-                   int64_t Lmax, int64_t L_cap, const float* rope, int64_t rope_npos, float theta, int pos_offset,
-                   float* gmax, float scale, const int64_t* len_dev, int64_t len_add, void* qtab, int64_t bstride,
-                   cudaStream_t st, const PageRef* pg) {
+int k_scores_batch(const AttendCall& c, const AttendScratch& s) {
+  const int H = c.Hq, B = c.B, grp = c.grp();
   int accumulate = 0;
-  if (outliers != nullptr) {
+  if (c.k_outliers != nullptr) {
     const size_t smem = (size_t)H * kHeadDim * sizeof(float2);
-    if (L_cap * n_out >= ((int64_t)1 << 31) || L_cap >= ((int64_t)1 << 25)) return KVQ_E_UNSUPPORTED;
-    const int sms = num_sms_cached();
-    k_batch_zero_kernel<<<dim3((unsigned)std::min<int64_t>((L_cap + 2047) / 2048, 64), H, B), 256, 0, st>>>(
-        scores, score_stride, bstride, len_dev, len_add, L_cap);
+    if (c.L * c.n_out >= ((int64_t)1 << 31) || c.L >= ((int64_t)1 << 25)) return KVQ_E_UNSUPPORTED;
+    k_batch_zero_kernel<<<dim3((unsigned)std::min<int64_t>((c.L + 2047) / 2048, 64), H, B), 256, 0, c.stream>>>(
+        s.scores, s.stride, s.bstride, c.len_dev, c.len_add, c.L);
     KVQ_LAUNCH_CHECK();
-    int rc = set_k_outlier_smem(smem, grp > 1, true, pg != nullptr);
+    const int rc = set_k_outlier_smem(smem, grp > 1, true, c.pg != nullptr);
     if (rc != 0) return rc;
-    // persistent CTAs as in launch_k_outliers, the per-SM allowance shared among the B sequences
-    const int64_t want = (L_cap * n_out + kOutPersThreads - 1) / kOutPersThreads;
-    const int per_sm = smem > 56 * 1024 ? 2 : 4;
-    const int64_t cap = std::max<int64_t>(1, (int64_t)sms * per_sm / B);
-    const dim3 grid((unsigned)std::max<int64_t>(1, std::min(want, cap)), (unsigned)B);
-    const float direct_theta = k_out_direct(L_cap + pos_offset) ? theta : 0.f;
-    const int64_t b_rows = Lmax * n_out;
-    if (pg != nullptr) {
-      if (grp > 1)
-        k_outlier_pers_kernel<true, true, true><<<grid, kOutPersThreads, smem, st>>>(
-            q, outliers, outlier_idx, scores, score_stride, 1, L_cap, H, n_out, reinterpret_cast<const float2*>(rope),
-            rope_npos, pos_offset, 1.f, len_dev, len_add, nullptr, direct_theta, grp, bstride, 0, *pg);
-      else
-        k_outlier_pers_kernel<false, true, true><<<grid, kOutPersThreads, smem, st>>>(
-            q, outliers, outlier_idx, scores, score_stride, 1, L_cap, H, n_out, reinterpret_cast<const float2*>(rope),
-            rope_npos, pos_offset, 1.f, len_dev, len_add, nullptr, direct_theta, 1, bstride, 0, *pg);
-    } else if (grp > 1)
-      k_outlier_pers_kernel<true, true><<<grid, kOutPersThreads, smem, st>>>(
-          q, outliers, outlier_idx, scores, score_stride, 1, L_cap, H, n_out, reinterpret_cast<const float2*>(rope),
-          rope_npos, pos_offset, 1.f, len_dev, len_add, nullptr, direct_theta, grp, bstride, b_rows, PageRef{});
-    else
-      k_outlier_pers_kernel<false, true><<<grid, kOutPersThreads, smem, st>>>(
-          q, outliers, outlier_idx, scores, score_stride, 1, L_cap, H, n_out, reinterpret_cast<const float2*>(rope),
-          rope_npos, pos_offset, 1.f, len_dev, len_add, nullptr, direct_theta, 1, bstride, b_rows, PageRef{});
+    const dim3 grid(k_outlier_grid(c.L * c.n_out, smem, B), (unsigned)B);
+    const float direct_theta = k_out_direct(c.L + c.pos_offset) ? c.theta : 0.f;
+    const int64_t b_rows = c.pg != nullptr ? 0 : c.Lmax * c.n_out;   // a pool has no per-sequence row block
+    with_flavour(grp > 1, true, c.pg != nullptr, [&](auto GQA, auto BATCH, auto PAGED) {
+      k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem, c.stream>>>(
+          c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, reinterpret_cast<const float2*>(c.rope),
+          c.rope_npos, c.pos_offset, 1.f, c.len_dev, c.len_add, nullptr, direct_theta, grp, s.bstride, b_rows,
+          c.pg != nullptr ? *c.pg : PageRef{});
+    });
     KVQ_LAUNCH_CHECK();
     accumulate = 1;
   }
-  return k_ratio_dispatch(bits, q, cache, scores, score_stride, lut, H, grp, Lmax, L_cap, rope, rope_npos, pos_offset, gmax,
-                          scale, accumulate, len_dev, len_add, qtab, 0, 1, st, B, bstride, pg);
+  return k_ratio_dispatch(c, s, 0, c.L, 1, accumulate);
 }
 
 }  // namespace kvq

@@ -67,18 +67,5 @@ inline int64_t k_token_range(int64_t L, int64_t splits) {
 int k_pair_dispatch(int bits, const KParams& p, cudaStream_t st);
 // dense K-score kernel, 3-bit, carried words (kvq_k3.cu)
 int k_scores3_dispatch(const KParams& p, cudaStream_t st);
-// dense K-score kernel of the fused attend, exact fp32 ratio form (kvq_kratio.cu).  B >= 1: a batch of B sequences
-// (len_dev[B]; q [B][H][128]; cache [B][Hkv*W][Lmax]; scores, gmax and qtab of sequence b at b * bstride floats).
-// pg != nullptr (with B >= 1): cache is the page pool [n_pool][Hkv*W][P] of a paged batch, Lmax unused.
-int k_ratio_dispatch(int bits, const float* q, const int32_t* cache, float* scores, int64_t score_stride, const float* lut,
-                     int H, int grp, int64_t Lmax, int64_t L, const float* rope, int64_t rope_npos, int pos_offset,
-                     float* gmax, float scale, int accumulate, const int64_t* len_dev, int64_t len_add, void* qtab,
-                     int64_t t0, int run_prep, cudaStream_t st, int B = 0, int64_t bstride = 0,
-                     const PageRef* pg = nullptr);
-// dense K-score kernel of the fused attend, fp16-table form (kvq_kfast.cu)
-int k_fast_dispatch(int bits, const float* q, const int32_t* cache, float* scores, int64_t score_stride, const float* lut,
-                    int H, int64_t Lmax, int64_t L, const void* rope_half, int64_t rope_npos, int pos_offset, float* gmax,
-                    float scale, int accumulate, const int64_t* len_dev, int64_t len_add, void* qtab, int64_t t0,
-                     int run_prep, cudaStream_t st);
 
 }  // namespace kvq

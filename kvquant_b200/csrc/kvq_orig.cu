@@ -153,8 +153,6 @@ __global__ void __launch_bounds__(kSpmvThreads) csc_v_spmv_kernel(
   }
 }
 
-int num_sms_cached();
-
 }  // namespace kvq
 
 using namespace kvq;

@@ -75,8 +75,6 @@ static int copy_side(const kvq_seq_ref* r, CopySide* s, int P, int64_t s1) {
   return 0;
 }
 
-int num_sms_cached();
-
 }  // namespace kvq
 
 using namespace kvq;

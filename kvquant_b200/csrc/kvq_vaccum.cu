@@ -7,9 +7,8 @@
 //
 //   O[h,c] = sum_t w[h,t] * (LUT[t, code(h,c,t)] (+) outlier(h,c,t))
 //
-// This file: the generic per-token-LUT kernel (legacy op surface, and the fused path over a cache given as
-// materialised LUT rows only), the attend_init / attend_combine / attend_merge kernels, the TMA descriptor helper
-// and the kvq_attend entry points.  The native fused-path V kernel is kvq_vnative.cu.
+// This file: the generic per-token-LUT kernel (legacy op surface kvq_v_matvec, and the fused attend over a cache given
+// as materialised LUT rows only).  The native fused-path V kernel is kvq_vnative.cu, the attend itself kvq_attend.cu.
 //
 // Design (DESIGN.md section 4.2):
 //   * one CTA streams a contiguous token range for ALL heads: the [H*W rows x 32 tokens] code slab of a tile is
@@ -26,10 +25,7 @@
 //     consecutive words: conflict-free;
 //   * outliers scatter into a shared-memory accumulator (42 shared atomics per token instead of 42 global
 //     atomics onto 4096 hot addresses).
-#include "kvq_common.cuh"
-#include <stdlib.h>
-#include <cuda_fp16.h>
-#include <dlfcn.h>
+#include "kvq_attend.cuh"
 
 namespace kvq {
 
@@ -362,163 +358,7 @@ __global__ void __launch_bounds__(kVThreads, 1) v_accum_kernel(const __grid_cons
   }
 }
 
-// ---- fused attend helpers ------------------------------------------------------------------------------------
-// sink scores (fp16 post-RoPE keys, modeling_llama.py:1948-1949) and the initial per-head max.  GQA: the sinks belong
-// to the cache, query head h reads those of KV head h / grp.
-// BATCH: sequence b = blockIdx.y of a batched attend: q [B][H][128], sink_k [B][H/grp][128][n_sink], sink scores and
-// maximum `bstride` floats after sequence b-1's.  BATCH = false ignores `bstride`.
-template <bool GQA, bool BATCH>
-__global__ void attend_init_kernel(const float* __restrict__ q, const __half* __restrict__ sink_k, int n_sink,
-                                   float* __restrict__ sink_scores, float* __restrict__ gmax, float scale, int grp,
-                                   const int64_t bstride) {
-  // grid = H, block = 128 (thread = channel): s_i = scale * sum_c q[h,c] * sink_k[h,c,i], reduced per sink
-  const int h = blockIdx.x, c = threadIdx.x;
-  const int hk = GQA ? h / grp : h;
-  if constexpr (BATCH) {
-    const int b = blockIdx.y;
-    q += (int64_t)b * gridDim.x * kHeadDim;
-    if (sink_k != nullptr) sink_k += (int64_t)b * (gridDim.x / grp) * kHeadDim * n_sink;
-    sink_scores += b * bstride;
-    gmax += b * bstride;
-  }
-  __shared__ float s_part[4];
-  __shared__ float s_max;
-  if (c == 0) s_max = -INFINITY;
-  const float qc = q[h * kHeadDim + c];
-  for (int i = 0; i < n_sink; ++i) {
-    float v = qc * __half2float(sink_k[((int64_t)hk * kHeadDim + c) * n_sink + i]);
-    v = warp_sum(v);
-    __syncthreads();
-    if ((c & 31) == 0) s_part[c >> 5] = v;
-    __syncthreads();
-    if (c == 0) {
-      const float s = (s_part[0] + s_part[1] + s_part[2] + s_part[3]) * scale;
-      sink_scores[h * 64 + i] = s;
-      s_max = fmaxf(s_max, s);
-    }
-  }
-  __syncthreads();
-  if (c == 0) gmax[h] = s_max;
-}
-
-// out[h,c] = (sum_s o[s,h,c] + sum_i p_i * sink_v[h,i,c]) / (sum_s l[s,h] + sum_i p_i),  p_i = exp(sink_s[h,i]-max)
-// grid = H, block = 1024: 32 slices of the partials (one warp each, a lane owns 4 channels: 16-byte loads, all of a
-// thread's <= 8 loads in flight at once), reduced through shared memory
-// GQA: sink_v of KV head h / grp
-// BATCH: sequence b = blockIdx.y of a batched attend: partials, maximum and sink scores `bstride` floats after sequence
-// b-1's, sink_v [B][H/grp][n_sink][128], out [B][H][128], out_lse [B][H].  A sequence with no slot and no sink (an idle
-// serving slot: l == 0) writes out = 0 and lse = -inf.  BATCH = false ignores `bstride`.
-template <bool GQA, bool BATCH>
-__global__ void __launch_bounds__(1024) attend_combine_kernel(const float* __restrict__ po, const float* __restrict__ pl,
-                                                              int n_part, int H, const float* __restrict__ gmax,
-                                                              const float* __restrict__ sink_scores,
-                                                              const __half* __restrict__ sink_v, int n_sink,
-                                                              float* __restrict__ out, float* __restrict__ out_lse,
-                                                              int grp, const int64_t bstride) {
-  __shared__ float4 s_o[32][32];
-  __shared__ float s_l[32];
-  const int h = blockIdx.x, lane = threadIdx.x & 31, g = threadIdx.x >> 5;
-  if constexpr (BATCH) {
-    const int b = blockIdx.y;
-    po += b * bstride; pl += b * bstride; gmax += b * bstride; sink_scores += b * bstride;
-    if (sink_v != nullptr) sink_v += (int64_t)b * (H / grp) * n_sink * kHeadDim;
-    out += (int64_t)b * H * kHeadDim;
-    if (out_lse != nullptr) out_lse += (int64_t)b * H;
-  }
-  float4 o4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  float lsum = 0.f;
-  constexpr int kU = 8;   // n_part <= 256 partials -> at most 8 per slice
-  float4 v[kU];
-  float lv[kU];
-#pragma unroll
-  for (int i = 0; i < kU; ++i) {
-    const int s = g + 32 * i;
-    v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    lv[i] = 0.f;
-    if (s < n_part) {
-      v[i] = __ldcg(reinterpret_cast<const float4*>(po + ((int64_t)s * H + h) * kHeadDim) + lane);
-      if (lane == 0) lv[i] = __ldcg(pl + (int64_t)s * H + h);
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < kU; ++i) { o4.x += v[i].x; o4.y += v[i].y; o4.z += v[i].z; o4.w += v[i].w; lsum += lv[i]; }
-  s_o[g][lane] = o4;
-  if (lane == 0) s_l[g] = lsum;
-  __syncthreads();
-  if (threadIdx.x >= kHeadDim) return;
-  const int c = threadIdx.x;
-  float o = 0.f, l = 0.f;
-#pragma unroll
-  for (int i = 0; i < 32; ++i) { o += reinterpret_cast<const float*>(&s_o[i][0])[c]; l += s_l[i]; }
-  float m = gmax[h];
-  for (int i = 0; i < n_sink; ++i) {
-    const float pi = __expf(sink_scores[h * 64 + i] - m);
-    o = fmaf(pi, __half2float(sink_v[((int64_t)(GQA ? h / grp : h) * n_sink + i) * kHeadDim + c]), o);
-    l += pi;
-  }
-  if (BATCH && l == 0.f) o = 0.f, l = 1.f, m = -INFINITY;   // idle slot: nothing attended
-  out[h * kHeadDim + c] = o / l;
-  if (out_lse != nullptr && c == 0) out_lse[h] = m + __logf(l);   // log-sum-exp of the scaled scores (for cross-GPU merges)
-}
-
-// merge N partial attention results (sequence-sharded decode): parts [N][H*128 + H] = (normalised out[H,128], lse[H])
-__global__ void attend_merge_kernel(const float* __restrict__ parts, int n, int H, float* __restrict__ out) {
-  const int h = blockIdx.x, c = threadIdx.x;   // block = 128
-  const int stride = H * kHeadDim + H;
-  float m = -INFINITY;
-  for (int r = 0; r < n; ++r) m = fmaxf(m, parts[(int64_t)r * stride + H * kHeadDim + h]);
-  float o = 0.f, l = 0.f;
-  for (int r = 0; r < n; ++r) {
-    const float* pr = parts + (int64_t)r * stride;
-    const float w = __expf(pr[H * kHeadDim + h] - m);
-    o = fmaf(w, pr[h * kHeadDim + c], o);
-    l += w;
-  }
-  out[h * kHeadDim + c] = o / l;
-}
-
 // ---- host side -----------------------------------------------------------------------------------------------
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int make_cache_tensor_map(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint32_t box_cols,
-                          uint32_t box_rows, int swizzle_bytes) {
-  static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
-    // resolve the driver entry point directly (no link-time dependency on libcuda; the library must load on
-    // GPU-less build hosts so that its exports can be checked there)
-    void* h = dlopen("libcuda.so.1", RTLD_NOW | RTLD_GLOBAL);
-    if (!h) return (int)cudaErrorInsufficientDriver;
-    void* sym = dlsym(h, "cuTensorMapEncodeTiled");
-    if (!sym) return (int)cudaErrorNotSupported;
-    fn = reinterpret_cast<PFN_encodeTiled>(sym);
-  }
-  const cuuint64_t gdim[2] = {cols, rows};
-  const cuuint64_t gstride[1] = {cols * 4};
-  const cuuint32_t box[2] = {box_cols, box_rows};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, const_cast<void*>(base), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE),
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : (int)cudaErrorInvalidValue;
-}
-
-static int g_sms[64];   // per device (one process may drive several GPUs, see PerDeviceOnce)
-int num_sms_cached();
-static int num_sms() { return num_sms_cached(); }
-int num_sms_cached() {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  int& n = g_sms[dev & 63];
-  if (!n) {
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
-}
-
 constexpr uint32_t kSmemBudget = 227u * 1024u;
 
 // ring stages that fit next to the LUT rows, weights and outlier accumulator for a slab of Hg heads (largest
@@ -565,7 +405,7 @@ static int launch_v(VParams p, const int32_t* cache, int* n_cta_out, cudaStream_
   if (rc != 0) return rc;
   // token ranges x head groups ~ one CTA per SM; the partial index is the token range
   const int64_t n_tiles = (p.L + kVT - 1) / kVT;
-  const int ranges = max(1, num_sms() / G);
+  const int ranges = max(1, num_sms_cached() / G);
   p.tiles_per_cta = (int)((n_tiles + ranges - 1) / ranges);
   const int n_cta = (int)((n_tiles + p.tiles_per_cta - 1) / p.tiles_per_cta);
   const dim3 grid(n_cta, G);
@@ -576,7 +416,7 @@ static int launch_v(VParams p, const int32_t* cache, int* n_cta_out, cudaStream_
   return 0;
 }
 
-int v_accum_dispatch(int bits, const VParams& p, const int32_t* cache, int* n_cta, cudaStream_t st) {
+static int v_accum_dispatch(int bits, const VParams& p, const int32_t* cache, int* n_cta, cudaStream_t st) {
   switch (bits) {
     case 4: return launch_v<4>(p, cache, n_cta, st);
     case 3: return launch_v<3>(p, cache, n_cta, st);
@@ -585,50 +425,22 @@ int v_accum_dispatch(int bits, const VParams& p, const int32_t* cache, int* n_ct
   }
 }
 
-struct KParams;  // kvq_kscore.cu
-int k_scores_fused(int bits, const float* q, const int32_t* cache, float* scores, int64_t score_stride,
-                   const float* lut, const float* outliers, const int32_t* outlier_idx, int n_out, int H,
-                   int64_t Lmax, int64_t L, const float* rope, int64_t rope_npos, float theta, int pos_offset,
-                   float* gmax, float scale, const int64_t* len_dev, int64_t len_add, float* opart, int opart_stride,
-                   cudaStream_t st);
-
-int v_native_dispatch(int bits, const float* score, int64_t score_stride, const float* gmax, const int32_t* cache,
-                      const float* v_cent, const float* v_aff, const float* outliers, const int32_t* outlier_idx,
-                      int n_out, int H, int grp, int64_t Lmax, int64_t L, float* out_o, float* out_l, int* n_cta,
-                      const int64_t* len_dev, int64_t len_add, cudaStream_t st, int B = 0, int64_t bstride = 0,
-                      const PageRef* pg = nullptr);
-int k_scores_batch(int bits, int B, const float* q, const int32_t* cache, float* scores, int64_t score_stride,
-                   const float* lut, const float* outliers, const int32_t* outlier_idx, int n_out, int H, int grp,
-                   int64_t Lmax, int64_t L_cap, const float* rope, int64_t rope_npos, float theta, int pos_offset,
-                   float* gmax, float scale, const int64_t* len_dev, int64_t len_add, void* qtab, int64_t bstride,
-                   cudaStream_t st, const PageRef* pg);
-
-int k_scores_fused_fast(int bits, const float* q, const int32_t* cache, float* scores, int64_t score_stride,
-                        const float* lut, const float* outliers, const int32_t* outlier_idx, int n_out, int H, int grp,
-                        int64_t Lmax, int64_t L, const float* rope, const void* rope_half, int64_t rope_npos, float theta,
-                        int pos_offset, float* gmax, float scale, const int64_t* len_dev, int64_t len_add, void* qtab,
-                        cudaStream_t st);
-// KVQ_K_IMPL set (generic / pair / kappa / lds64): round 1's 8-byte-entry kernels serve the exact mode of the fused attend
-static int k_legacy_fused() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("KVQ_K_IMPL"); v = (e && e[0]) ? 1 : 0; }
-  return v;
-}
-
-static int check_v_common(int H, int64_t Lmax, int64_t L, const void* cache) {
-  if (H <= 0 || (H & 3) != 0 || H > 64 || L < 0 || L > Lmax) return KVQ_E_SHAPE;
-  if ((Lmax & 3) != 0 || (reinterpret_cast<uintptr_t>(cache) & 15) != 0) return KVQ_E_ALIGN;
-  return 0;
+// the fused attend over a cache given as materialised LUT rows only (kvq_attend without v_cent / v_aff)
+int v_accum_fused(const AttendCall& c, const AttendScratch& s, int* n_cta) {
+  VParams p{};
+  p.score = s.scores; p.lut_tok = c.vlut_tok; p.out = s.part_o; p.out_l = s.part_l; p.gmax = s.gmax;
+  p.outliers = c.v_outliers; p.outlier_idx = c.v_outlier_idx;
+  p.Lmax = c.Lmax; p.L = c.L; p.score_stride = s.stride; p.H = c.Hq; p.n_out = c.n_out; p.fused = 1;
+  return v_accum_dispatch(c.bits, p, c.vcache, n_cta, c.stream);
 }
 
 }  // namespace kvq
 
 using namespace kvq;
 
-extern "C" {
-
-int kvq_v_matvec(int bits, const float* score, const int32_t* cache, float* mul, const float* lut_tok, int B, int H,
-                 int64_t Lmax, int64_t L, const float* outliers, const int32_t* outlier_idx, int n_out, void* stream) {
+extern "C" int kvq_v_matvec(int bits, const float* score, const int32_t* cache, float* mul, const float* lut_tok, int B,
+                            int H, int64_t Lmax, int64_t L, const float* outliers, const int32_t* outlier_idx, int n_out,
+                            void* stream) {
   if (!score || !cache || !mul || !lut_tok) return KVQ_E_NULL;
   if (B <= 0) return KVQ_E_SHAPE;
   int rc = check_v_common(H, Lmax, L, cache);
@@ -652,259 +464,3 @@ int kvq_v_matvec(int bits, const float* score, const int32_t* cache, float* mul,
   }
   return 0;
 }
-
-static int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
-static const int kMaxPart = 256;
-
-int64_t kvq_attend_scratch_bytes(int H, int64_t L) {
-  // scores [H][L'] + gmax [H] + sink scores [H][64] + partial o / l of <= kMaxPart CTAs + token-major K-outlier
-  // partials [L'][H'] (H' = H rounded up to 32) + the premultiplied K table [H][128][16] and ratios [H][128]
-  return 4 * ((int64_t)H * round_up(L, 32) + H + (int64_t)H * 64 + (int64_t)kMaxPart * H * kHeadDim + (int64_t)kMaxPart * H +
-              round_up(L, 32) * round_up(H, 32) + (int64_t)H * kHeadDim * 17) + 256;
-}
-
-}  // extern "C"
-
-static int attend_impl(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-               const int32_t* k_outlier_idx, const int32_t* vcache, const float* vlut_tok, const float* v_cent,
-               const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int H, int64_t Lmax, int64_t L, const float* rope_cos_sin,
-               int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
-               float* out, float* out_lse, void* scratch, const int64_t* len_dev, int64_t len_add, const void* rope_half,
-               void* stream, int grp = 1) {
-  // H: query heads; grp of them per KV head (the caches, tables, outlier rows and sinks hold H / grp heads)
-  if (!q || !kcache || !klut || !vcache || !rope_cos_sin || !out || !scratch) return KVQ_E_NULL;
-  const bool native_v = (v_cent != nullptr && v_aff != nullptr);
-  if (!native_v && !vlut_tok) return KVQ_E_NULL;
-  int rc = check_v_common(H, Lmax, L, vcache);
-  if (rc) return rc;
-  if ((k_outliers == nullptr) != (k_outlier_idx == nullptr) || (v_outliers == nullptr) != (v_outlier_idx == nullptr)) return KVQ_E_NULL;
-  if ((k_outliers || v_outliers) && n_out <= 0) return KVQ_E_SHAPE;
-  if (n_sink < 0 || n_sink > 64 || (n_sink > 0 && (!sink_k || !sink_v))) return KVQ_E_SHAPE;
-  if (L + n_sink == 0 || rope_npos < L + pos_offset || Lmax >= ((int64_t)1 << 30)) return KVQ_E_SHAPE;
-  if (num_sms() > kMaxPart) return KVQ_E_UNSUPPORTED;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int64_t stride = round_up(L, 32);
-  float* scores = static_cast<float*>(scratch);
-  float* gmax = scores + (int64_t)H * stride;
-  float* sink_scores = gmax + H;
-  float* part_o = sink_scores + (int64_t)H * 64;
-  float* part_l = part_o + (int64_t)kMaxPart * H * kHeadDim;
-  float* opart = part_l + (int64_t)kMaxPart * H;          // 16-byte aligned: every block above is a multiple of 4 floats
-  const int opart_stride = (int)round_up(H, 32);
-  float* qtab = opart + round_up(L, 32) * opart_stride;    // 16-byte aligned (rows of 32 floats)
-  const bool fast = rope_half != nullptr;                  // fp16 tables (north_star's precision); NULL = exact fp32
-  const float scale = 0.08838834764831845f;  // 1/sqrt(128)  (modeling_llama.py:1959,1973)
-  if (grp > 1) attend_init_kernel<true, false><<<H, kHeadDim, 0, st>>>(q, static_cast<const __half*>(sink_k), n_sink, sink_scores, gmax, scale, grp, 0);
-  else attend_init_kernel<false, false><<<H, kHeadDim, 0, st>>>(q, static_cast<const __half*>(sink_k), n_sink, sink_scores, gmax, scale, 1, 0);
-  KVQ_LAUNCH_CHECK();
-  int n_cta = 0;
-  if (L > 0) {
-    // KVQ_K_IMPL (generic / pair / kappa) keeps round 1's LDS.64 kernels reachable for A/B runs; otherwise the
-    // TMA-fed kernels: exact fp32 ratio form, or (rope_half given) the fp16-table form
-    if (!fast && k_legacy_fused())
-      rc = k_scores_fused(bits, q, kcache, scores, stride, klut, k_outliers, k_outlier_idx, n_out, H, Lmax, L,
-                          rope_cos_sin, rope_npos, theta, pos_offset, gmax, scale, len_dev, len_add, opart, opart_stride, st);
-    else
-      rc = k_scores_fused_fast(bits, q, kcache, scores, stride, klut, k_outliers, k_outlier_idx, n_out, H, grp, Lmax, L,
-                               rope_cos_sin, rope_half, rope_npos, theta, pos_offset, gmax, scale, len_dev, len_add, qtab, st);
-    if (rc) return rc;
-    if (native_v) {
-      rc = v_native_dispatch(bits, scores, stride, gmax, vcache, v_cent, v_aff, v_outliers, v_outlier_idx, n_out, H, grp,
-                             Lmax, L, part_o, part_l, &n_cta, len_dev, len_add, st);
-    } else {   // materialised per-token LUT rows (kvq_attend without v_cent / v_aff)
-      VParams p{};
-      p.score = scores; p.lut_tok = vlut_tok; p.out = part_o; p.out_l = part_l; p.gmax = gmax;
-      p.outliers = v_outliers; p.outlier_idx = v_outlier_idx;
-      p.Lmax = Lmax; p.L = L; p.score_stride = stride; p.H = H; p.n_out = n_out; p.fused = 1;
-      rc = v_accum_dispatch(bits, p, vcache, &n_cta, st);
-    }
-    if (rc) return rc;
-  }
-  if (grp > 1)
-    attend_combine_kernel<true, false><<<H, 1024, 0, st>>>(part_o, part_l, n_cta, H, gmax, sink_scores,
-                                                    static_cast<const __half*>(sink_v), n_sink, out, out_lse, grp, 0);
-  else
-    attend_combine_kernel<false, false><<<H, 1024, 0, st>>>(part_o, part_l, n_cta, H, gmax, sink_scores,
-                                                     static_cast<const __half*>(sink_v), n_sink, out, out_lse, 1, 0);
-  KVQ_LAUNCH_CHECK();
-  return 0;
-}
-
-extern "C" {
-
-int kvq_attend(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-               const int32_t* k_outlier_idx, const int32_t* vcache, const float* vlut_tok, const float* v_cent,
-               const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int H, int64_t Lmax, int64_t L, const float* rope_cos_sin,
-               int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
-               float* out, float* out_lse, void* scratch, const void* rope_half, void* stream) {
-  return attend_impl(bits, q, kcache, klut, k_outliers, k_outlier_idx, vcache, vlut_tok, v_cent, v_aff, v_outliers,
-                     v_outlier_idx, n_out, H, Lmax, L, rope_cos_sin, rope_npos, theta, pos_offset, sink_k, sink_v, n_sink,
-                     out, out_lse, scratch, nullptr, 0, rope_half, stream);
-}
-
-int kvq_attend_dyn(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-                   const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
-                   const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int H, int64_t Lmax, int64_t L_cap,
-                   const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin, int64_t rope_npos, float theta,
-                   int pos_offset, const void* sink_k, const void* sink_v, int n_sink, float* out, float* out_lse,
-                   void* scratch, const void* rope_half, void* stream) {
-  if (!len_dev || !v_cent || !v_aff) return KVQ_E_NULL;
-  if (L_cap <= 0) return KVQ_E_SHAPE;
-  return attend_impl(bits, q, kcache, klut, k_outliers, k_outlier_idx, vcache, nullptr, v_cent, v_aff, v_outliers,
-                     v_outlier_idx, n_out, H, Lmax, L_cap, rope_cos_sin, rope_npos, theta, pos_offset, sink_k, sink_v,
-                     n_sink, out, out_lse, scratch, len_dev, len_add, rope_half, stream);
-}
-
-// Grouped-query attention: Hq query heads over an Hkv-head cache, query head h attending over KV head h / (Hq / Hkv).
-// Hq == Hkv is kvq_attend itself; otherwise the exact-table, native-V path only.
-static int check_gqa(int Hq, int Hkv) {
-  if (Hkv <= 0 || Hq <= 0 || Hq > 64 || (Hq & 3) != 0 || (Hkv & 3) != 0 || Hq % Hkv != 0) return KVQ_E_SHAPE;
-  return 0;
-}
-static int gqa_unsupported(const float* v_cent, const float* v_aff, const void* rope_half) {
-  return (v_cent == nullptr || v_aff == nullptr || rope_half != nullptr || k_legacy_fused()) ? KVQ_E_UNSUPPORTED : 0;
-}
-
-int kvq_attend_gqa(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-                   const int32_t* k_outlier_idx, const int32_t* vcache, const float* vlut_tok, const float* v_cent,
-                   const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv,
-                   int64_t Lmax, int64_t L, const float* rope_cos_sin, int64_t rope_npos, float theta, int pos_offset,
-                   const void* sink_k, const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
-                   const void* rope_half, void* stream) {
-  int rc = check_gqa(Hq, Hkv);
-  if (rc) return rc;
-  if (Hq == Hkv)
-    return kvq_attend(bits, q, kcache, klut, k_outliers, k_outlier_idx, vcache, vlut_tok, v_cent, v_aff, v_outliers,
-                      v_outlier_idx, n_out, Hq, Lmax, L, rope_cos_sin, rope_npos, theta, pos_offset, sink_k, sink_v,
-                      n_sink, out, out_lse, scratch, rope_half, stream);
-  if ((rc = gqa_unsupported(v_cent, v_aff, rope_half)) != 0) return rc;
-  return attend_impl(bits, q, kcache, klut, k_outliers, k_outlier_idx, vcache, nullptr, v_cent, v_aff, v_outliers,
-                     v_outlier_idx, n_out, Hq, Lmax, L, rope_cos_sin, rope_npos, theta, pos_offset, sink_k, sink_v, n_sink,
-                     out, out_lse, scratch, nullptr, 0, nullptr, stream, Hq / Hkv);
-}
-
-int kvq_attend_gqa_dyn(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-                       const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
-                       const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax,
-                       int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
-                       int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
-                       float* out, float* out_lse, void* scratch, const void* rope_half, void* stream) {
-  int rc = check_gqa(Hq, Hkv);
-  if (rc) return rc;
-  if (Hq == Hkv)
-    return kvq_attend_dyn(bits, q, kcache, klut, k_outliers, k_outlier_idx, vcache, v_cent, v_aff, v_outliers,
-                          v_outlier_idx, n_out, Hq, Lmax, L_cap, len_dev, len_add, rope_cos_sin, rope_npos, theta,
-                          pos_offset, sink_k, sink_v, n_sink, out, out_lse, scratch, rope_half, stream);
-  if ((rc = gqa_unsupported(v_cent, v_aff, rope_half)) != 0) return rc;
-  if (!len_dev) return KVQ_E_NULL;
-  if (L_cap <= 0) return KVQ_E_SHAPE;
-  return attend_impl(bits, q, kcache, klut, k_outliers, k_outlier_idx, vcache, nullptr, v_cent, v_aff, v_outliers,
-                     v_outlier_idx, n_out, Hq, Lmax, L_cap, rope_cos_sin, rope_npos, theta, pos_offset, sink_k, sink_v,
-                     n_sink, out, out_lse, scratch, len_dev, len_add, nullptr, stream, Hq / Hkv);
-}
-
-// Batched decode attend: B sequences of one layer in one launch set (init -> prep -> K outliers -> K ratio -> V native
-// -> combine), the sequence a grid dimension.  Sequence b's scratch block is bytes [b*S, (b+1)*S) of scratch, S =
-// kvq_attend_scratch_bytes(Hq, L_cap) (a multiple of 16 bytes), laid out as the single-sequence call lays it out.
-int64_t kvq_attend_batch_scratch_bytes(int B, int Hq, int64_t L_cap) {
-  if (B < 1 || B > 256 || Hq <= 0 || L_cap <= 0) return 0;
-  return (int64_t)B * kvq_attend_scratch_bytes(Hq, L_cap);
-}
-
-// pg == nullptr: kvq_attend_batch over a batch-strided cache of Lmax slots per sequence; else kvq_attend_paged, Lmax
-// = max_pages * P (the per-sequence cap) and the caches and row tensors page pools.  Init, prep, score clear and combine
-// work on logical token indices in the scratch, so they are the same for both; only the kernels that read the cache
-// (K outliers, K ratio, V native) look pages up.  The grids are sized by (B, Hq, L_cap) alone, so a paged call runs
-// the contiguous call's grids.
-static int attend_batch_impl(int bits, int B, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-                             const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
-                             const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax,
-                             int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
-                             int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
-                             float* out, float* out_lse, void* scratch, const void* rope_half, void* stream,
-                             const PageRef* pg) {
-  int rc = check_gqa(Hq, Hkv);
-  if (rc) return rc;
-  if (B < 1 || B > 256 || L_cap <= 0) return KVQ_E_SHAPE;
-  if (bits < 2 || bits > 4) return KVQ_E_BITS;
-  if ((rc = gqa_unsupported(v_cent, v_aff, rope_half)) != 0) return rc;
-  if (!q || !kcache || !klut || !vcache || !rope_cos_sin || !out || !scratch || !len_dev) return KVQ_E_NULL;
-  if (pg != nullptr && (!pg->table || !pg->npages)) return KVQ_E_NULL;
-  if (pg != nullptr && (rc = check_pages(pg->n_pool, pg->max_pages, pg->P, (int64_t)Hkv * kHeadDim * bits / 32)) != 0) return rc;
-  if ((rc = check_v_common(Hq, Lmax, L_cap, vcache)) != 0) return rc;
-  if ((reinterpret_cast<uintptr_t>(kcache) & 15) != 0 || (reinterpret_cast<uintptr_t>(scratch) & 15) != 0) return KVQ_E_ALIGN;
-  if ((k_outliers == nullptr) != (k_outlier_idx == nullptr) || (v_outliers == nullptr) != (v_outlier_idx == nullptr)) return KVQ_E_NULL;
-  if ((k_outliers || v_outliers) && n_out <= 0) return KVQ_E_SHAPE;
-  if (n_sink < 0 || n_sink > 64 || (n_sink > 0 && (!sink_k || !sink_v))) return KVQ_E_SHAPE;
-  if (rope_npos < L_cap + pos_offset || pos_offset < 0 || Lmax >= ((int64_t)1 << 30)) return KVQ_E_SHAPE;
-  if (num_sms() > kMaxPart) return KVQ_E_UNSUPPORTED;
-  const int grp = Hq / Hkv, H = Hq;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int64_t bstride = kvq_attend_scratch_bytes(H, L_cap) / 4;   // floats per sequence block
-  const int64_t stride = round_up(L_cap, 32);
-  // the offsets of attend_impl's carve-up, inside sequence 0's block; the kernels add b * bstride
-  float* scores = static_cast<float*>(scratch);
-  float* gmax = scores + (int64_t)H * stride;
-  float* sink_scores = gmax + H;
-  float* part_o = sink_scores + (int64_t)H * 64;
-  float* part_l = part_o + (int64_t)kMaxPart * H * kHeadDim;
-  float* opart = part_l + (int64_t)kMaxPart * H;
-  float* qtab = opart + round_up(L_cap, 32) * round_up(H, 32);
-  const float scale = 0.08838834764831845f;  // 1/sqrt(128)
-  const __half* sk = static_cast<const __half*>(sink_k);
-  if (grp > 1) attend_init_kernel<true, true><<<dim3(H, B), kHeadDim, 0, st>>>(q, sk, n_sink, sink_scores, gmax, scale, grp, bstride);
-  else attend_init_kernel<false, true><<<dim3(H, B), kHeadDim, 0, st>>>(q, sk, n_sink, sink_scores, gmax, scale, 1, bstride);
-  KVQ_LAUNCH_CHECK();
-  rc = k_scores_batch(bits, B, q, kcache, scores, stride, klut, k_outliers, k_outlier_idx, n_out, H, grp, Lmax, L_cap,
-                      rope_cos_sin, rope_npos, theta, pos_offset, gmax, scale, len_dev, len_add, qtab, bstride, st, pg);
-  if (rc) return rc;
-  int n_cta = 0;
-  rc = v_native_dispatch(bits, scores, stride, gmax, vcache, v_cent, v_aff, v_outliers, v_outlier_idx, n_out, H, grp,
-                         Lmax, L_cap, part_o, part_l, &n_cta, len_dev, len_add, st, B, bstride, pg);
-  if (rc) return rc;
-  const __half* sv = static_cast<const __half*>(sink_v);
-  if (grp > 1)
-    attend_combine_kernel<true, true><<<dim3(H, B), 1024, 0, st>>>(part_o, part_l, n_cta, H, gmax, sink_scores, sv, n_sink,
-                                                                   out, out_lse, grp, bstride);
-  else
-    attend_combine_kernel<false, true><<<dim3(H, B), 1024, 0, st>>>(part_o, part_l, n_cta, H, gmax, sink_scores, sv, n_sink,
-                                                                    out, out_lse, 1, bstride);
-  KVQ_LAUNCH_CHECK();
-  return 0;
-}
-
-int kvq_attend_batch(int bits, int B, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-                     const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
-                     const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax,
-                     int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
-                     int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
-                     float* out, float* out_lse, void* scratch, const void* rope_half, void* stream) {
-  return attend_batch_impl(bits, B, q, kcache, klut, k_outliers, k_outlier_idx, vcache, v_cent, v_aff, v_outliers,
-                           v_outlier_idx, n_out, Hq, Hkv, Lmax, L_cap, len_dev, len_add, rope_cos_sin, rope_npos, theta,
-                           pos_offset, sink_k, sink_v, n_sink, out, out_lse, scratch, rope_half, stream, nullptr);
-}
-
-// Paged batch: the argument list of kvq_attend_batch with the pool size n_pool in place of Lmax, plus the page table
-int kvq_attend_paged(int bits, int B, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-                     const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
-                     const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int n_pool,
-                     int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
-                     int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
-                     float* out, float* out_lse, void* scratch, const void* rope_half, void* stream,
-                     const int32_t* page_table, int max_pages, const int32_t* npages, int P) {
-  const PageRef pg{page_table, npages, max_pages, P, n_pool};
-  return attend_batch_impl(bits, B, q, kcache, klut, k_outliers, k_outlier_idx, vcache, v_cent, v_aff, v_outliers,
-                           v_outlier_idx, n_out, Hq, Hkv, (int64_t)max_pages * P, L_cap, len_dev, len_add, rope_cos_sin,
-                           rope_npos, theta, pos_offset, sink_k, sink_v, n_sink, out, out_lse, scratch, rope_half, stream,
-                           &pg);
-}
-
-int kvq_attend_merge(const float* parts, int n_parts, int H, float* out, void* stream) {
-  if (!parts || !out) return KVQ_E_NULL;
-  if (n_parts <= 0 || H <= 0) return KVQ_E_SHAPE;
-  attend_merge_kernel<<<H, kHeadDim, 0, static_cast<cudaStream_t>(stream)>>>(parts, n_parts, H, out);
-  KVQ_LAUNCH_CHECK();
-  return 0;
-}
-
-}  // extern "C"

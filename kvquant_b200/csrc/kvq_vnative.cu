@@ -24,7 +24,7 @@
 // heads' word rows, read from HBM once per token range; a thread unit is (query head, KV word row), so the g units of
 // one KV row read the same staged words with their own head's weights.  Each V outlier entry (a KV channel) is applied
 // with the weights of the grp query heads of its KV head.  A head-split CTA owns whole groups.
-#include "kvq_common.cuh"
+#include "kvq_attend.cuh"
 #include <stdlib.h>
 
 namespace kvq {
@@ -457,7 +457,6 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
 }
 
 constexpr uint32_t kVNSmemBudget = 227u * 1024u;
-int num_sms_cached();
 
 // ring stages that fit next to the table for a slab of Hg query heads, grp per KV head (largest first); 0 when not
 // even two do
@@ -486,22 +485,13 @@ static int launch_vn_kernel(const CUtensorMap& tmap, const VNParams& p, dim3 gri
   return 0;
 }
 
-// B == 0: one sequence; B >= 1: a batch (grid dimension z = sequence, each with its own scratch block of bstride
-// floats); PAGED: a paged batch
-template <int BITS, bool BATCH, bool PAGED = false>
-static int launch_vn_grid(const CUtensorMap& tmap, const VNParams& p, dim3 grid, int G, uint32_t smem, cudaStream_t st,
-                          int64_t bstride, const PageRef& pg = PageRef{}) {
-  if (p.grp > 1)
-    return G == 1 ? launch_vn_kernel<BITS, false, true, BATCH, PAGED>(tmap, p, grid, smem, st, bstride, pg)
-                  : launch_vn_kernel<BITS, true, true, BATCH, PAGED>(tmap, p, grid, smem, st, bstride, pg);
-  return G == 1 ? launch_vn_kernel<BITS, false, false, BATCH, PAGED>(tmap, p, grid, smem, st, bstride, pg)
-                : launch_vn_kernel<BITS, true, false, BATCH, PAGED>(tmap, p, grid, smem, st, bstride, pg);
-}
-
+// c.B == 0: one sequence; c.B >= 1: a batch (grid dimension z = sequence, each with its own scratch block of s.bstride
+// floats); c.pg != nullptr: a paged batch
 template <int BITS>
-static int launch_vn(VNParams p, const int32_t* cache, int* n_cta_out, cudaStream_t st, int B, int64_t bstride,
-                     const PageRef* pg) {
+static int launch_vn(VNParams p, const AttendCall& c, const AttendScratch& s, int* n_cta_out) {
   using C = VNCfg<BITS>;
+  const int B = c.B;
+  const bool batch = B > 0, paged = c.pg != nullptr;
   // G head groups: 1 while the whole slab fits (every shape up to 4-bit H = 32, 3-bit H = 56, 2-bit H = 64), else 2.
   // G = 2 always fits for H <= 64: Hg = H/2 <= 32 heads is at most the 7B slab, and H % 4 == 0 keeps Hg even, so
   // the 3-bit group rows (Hg*12) stay a multiple of 8 for the TMA box below.
@@ -521,40 +511,40 @@ static int launch_vn(VNParams p, const int32_t* cache, int* n_cta_out, cudaStrea
   p.box_rows = rows / nb;
   // a batch: one map over the B sequences' caches (sequence b's rows follow b*Hkv*W others); a paged batch: one map
   // over the pool (n_pool*Hkv*W rows of P tokens)
-  int rc = pg != nullptr
-      ? make_cache_tensor_map(&tmap, cache, (uint64_t)pg->n_pool * (p.H / p.grp) * C::W, (uint64_t)pg->P, kNT,
+  int rc = paged
+      ? make_cache_tensor_map(&tmap, c.vcache, (uint64_t)c.pg->n_pool * (p.H / p.grp) * C::W, (uint64_t)c.pg->P, kNT,
                               (uint32_t)p.box_rows, /*swizzle bytes*/ 128)
-      : make_cache_tensor_map(&tmap, cache, (uint64_t)(B > 0 ? B : 1) * (p.H / p.grp) * C::W, (uint64_t)p.Lmax, kNT,
+      : make_cache_tensor_map(&tmap, c.vcache, (uint64_t)(batch ? B : 1) * (p.H / p.grp) * C::W, (uint64_t)p.Lmax, kNT,
                               (uint32_t)p.box_rows, /*swizzle bytes*/ 128);
   if (rc != 0) return rc;
   // token ranges x head groups (x sequences) ~ one CTA per SM; the partial index is the token range
   const int64_t n_tiles = (p.L + kNT - 1) / kNT;
-  const int ranges = max(1, num_sms_cached() / (G * (B > 0 ? B : 1)));
+  const int ranges = max(1, num_sms_cached() / (G * (batch ? B : 1)));
   p.tiles_per_cta = (int)((n_tiles + ranges - 1) / ranges);
   const int n_cta = (int)((n_tiles + p.tiles_per_cta - 1) / p.tiles_per_cta);
-  rc = pg != nullptr ? launch_vn_grid<BITS, true, true>(tmap, p, dim3(n_cta, G, B), G, lay.total + 1024u, st, bstride, *pg)
-     : B > 0 ? launch_vn_grid<BITS, true>(tmap, p, dim3(n_cta, G, B), G, lay.total + 1024u, st, bstride)
-             : launch_vn_grid<BITS, false>(tmap, p, dim3(n_cta, G), G, lay.total + 1024u, st, 0);
+  const dim3 grid = batch ? dim3(n_cta, G, B) : dim3(n_cta, G);
+  const uint32_t smem = lay.total + 1024u;
+  const PageRef pg = paged ? *c.pg : PageRef{};
+  rc = with_flavour(p.grp > 1, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
+    return G == 1 ? launch_vn_kernel<BITS, false, GQA(), BATCH(), PAGED()>(tmap, p, grid, smem, c.stream, s.bstride, pg)
+                  : launch_vn_kernel<BITS, true, GQA(), BATCH(), PAGED()>(tmap, p, grid, smem, c.stream, s.bstride, pg);
+  });
   if (rc != 0) return rc;
   *n_cta_out = n_cta;
   return 0;
 }
 
-int v_native_dispatch(int bits, const float* score, int64_t score_stride, const float* gmax, const int32_t* cache,
-                      const float* v_cent, const float* v_aff, const float* outliers, const int32_t* outlier_idx,
-                      int n_out, int H, int grp, int64_t Lmax, int64_t L, float* out_o, float* out_l, int* n_cta,
-                      const int64_t* len_dev, int64_t len_add, cudaStream_t st, int B, int64_t bstride,
-                      const PageRef* pg) {
+int v_native_dispatch(const AttendCall& c, const AttendScratch& s, int* n_cta) {
   VNParams p{};
-  p.grp = grp;
-  p.len_dev = len_dev; p.len_add = len_add;
-  p.score = score; p.gmax = gmax; p.v_cent = v_cent; p.v_aff = v_aff; p.out_o = out_o; p.out_l = out_l;
-  p.outliers = outliers; p.outlier_idx = outlier_idx; p.Lmax = Lmax; p.L = L; p.score_stride = score_stride;
-  p.H = H; p.n_out = n_out;
-  switch (bits) {
-    case 4: return launch_vn<4>(p, cache, n_cta, st, B, bstride, pg);
-    case 3: return launch_vn<3>(p, cache, n_cta, st, B, bstride, pg);
-    case 2: return launch_vn<2>(p, cache, n_cta, st, B, bstride, pg);
+  p.grp = c.grp();
+  p.len_dev = c.len_dev; p.len_add = c.len_add;
+  p.score = s.scores; p.gmax = s.gmax; p.v_cent = c.v_cent; p.v_aff = c.v_aff; p.out_o = s.part_o; p.out_l = s.part_l;
+  p.outliers = c.v_outliers; p.outlier_idx = c.v_outlier_idx; p.Lmax = c.Lmax; p.L = c.L; p.score_stride = s.stride;
+  p.H = c.Hq; p.n_out = c.n_out;
+  switch (c.bits) {
+    case 4: return launch_vn<4>(p, c, s, n_cta);
+    case 3: return launch_vn<3>(p, c, s, n_cta);
+    case 2: return launch_vn<2>(p, c, s, n_cta);
     default: return KVQ_E_BITS;
   }
 }
