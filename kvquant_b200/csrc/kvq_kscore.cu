@@ -22,6 +22,7 @@
 #include "kvq_kscore.cuh"
 #include "kvq_attend.cuh"
 #include <cuda_fp16.h>
+#include <math_constants.h>
 #include <stdlib.h>
 #include <algorithm>
 
@@ -503,6 +504,19 @@ static int launch_k_kappa(const KParams& p, cudaStream_t st) {
 // ------------------------------------------------------------------------------------------------------------
 constexpr int kOutThreads = 256;
 
+// theta_j of rotary row j, and (cos, sin)(theta_j * pos): the reference's expressions (quant_cuda_kernel.cu:3081 and
+// 3123-3126).  The rope table is built from them and the outlier pass evaluates them, so both hold the same bits.
+__device__ __forceinline__ float rope_row_theta(float rope_theta, int j) {
+  const int headdim = kHeadDim;
+  const int headdim2 = headdim / 2;
+  return powf(rope_theta, (-2 * __int2float_rd(j % headdim2) / __int2float_rd(headdim)));
+}
+__device__ __forceinline__ float2 rope_cos_sin(float theta, int pos) {
+  const float c = cosf(theta * pos);
+  const float s = sinf(theta * pos);
+  return make_float2(c, s);
+}
+
 // thread = one (token, outlier slot) entry.  cos/sin come from the RoPE table (bit-identical to the reference's
 // cosf/sinf(theta*pos)); entries of one (token, head) are adjacent (rows are sorted by channel), so a warp-level
 // segmented sum leaves ~1 atomic per (token, head) instead of the reference's one per entry.
@@ -546,13 +560,13 @@ __global__ void __launch_bounds__(kOutThreads) k_outlier_kernel(
 
 // Persistent form (default).  ncu on the kernel above: load/store data path 75 % busy -- per ENTRY one scattered
 // 8-byte rope read plus TWO scattered reads of q.  Here CTAs are persistent and keep (q[c], q[c^64]) for all channels
-// in shared memory (one 8-byte shared read per entry instead of two scattered global ones); the rope values still
-// come from the table.  In the fused path the sums go to a TOKEN-major partial buffer (a token's heads share one
+// in shared memory (one 8-byte shared read per entry instead of two scattered global ones); the rotary factors are
+// computed (rope_theta > 0, k_out_direct) or gathered from the table.  In the fused path the sums go to a TOKEN-major partial buffer (a token's heads share one
 // 128-byte line, so a warp's ~25 reductions coalesce into one or two L1 requests).
 // Alternatives considered (DESIGN.md section 4.1): a second, token-major copy of the rope table read with coalesced
 // row loads + shuffles instead of the gather (it loads rows for the zero-valued pads too and adds 8 shuffles per
-// entry); evaluating cosf/sinf(theta_j * pos) per entry instead of the gather (more instructions; used beyond
-// L2-sized rope tables, k_out_direct); accumulating into a per-CTA [H][256-token] shared tile with coalesced write-out
+// entry); gathering every entry's rotary factors from the rope table (slower than computing them, even at 32K);
+// accumulating into a per-CTA [H][256-token] shared tile with coalesced write-out
 // instead of global atomics (shared-memory fp32 atomics are compare-and-swap loops).
 //
 // GQA (grp query heads per KV head, H = query heads): an entry's channel is a KV channel; it is read once and adds its
@@ -564,6 +578,7 @@ __global__ void __launch_bounds__(kOutThreads) k_outlier_kernel(
 // PAGED (with BATCH, b_rows = 0): the outlier rows are a page pool; logical entry e = t * n_out + k of sequence b is
 // read from row page_of(b, t) * P + t % P, and the length is also capped at npages[b] * P.  Others ignore `pg`.
 constexpr int kOutPersThreads = 512;
+constexpr size_t kOutThetaBytes = kHalf * sizeof(float);   // dynamic shared memory past the q table: s_th
 template <bool GQA, bool BATCH, bool PAGED = false>
 __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
     const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
@@ -572,6 +587,7 @@ __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
     const int64_t* __restrict__ len_dev, int64_t len_add, const uint32_t* __restrict__ rope_h, float rope_theta, int grp,
     const int64_t b_out, const int64_t b_rows, const PageRef pg) {
   extern __shared__ float2 s_qq[];                       // [H*128] = (q[c], q[c^64]), query heads
+  float* const s_th = reinterpret_cast<float*>(s_qq + H * kHeadDim);   // [64]: theta_j of rotary row j (rope_theta > 0)
   if constexpr (BATCH) {
     const int b = blockIdx.y;
     q += (int64_t)b * H * kHeadDim;
@@ -587,12 +603,14 @@ __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
     const int64_t cap = page_cap(pg, blockIdx.y);
     L = L < cap ? L : cap;
   }
+  const uint32_t total = (uint32_t)(L * n_out);          // host checks L * n_out < 2^31
   const int tid = threadIdx.x, lane = tid & 31;
   for (int i = tid; i < H * kHeadDim; i += kOutPersThreads) s_qq[i] = make_float2(q[i], q[i ^ kHalf]);
+  if (rope_theta > 0.f && tid < kHalf) s_th[tid] = rope_row_theta(rope_theta, tid);
   __syncthreads();
-  const uint32_t total = (uint32_t)(L * n_out);          // host checks L * n_out < 2^31
   const uint32_t stride = gridDim.x * kOutPersThreads;
-  const uint64_t pol_keep = policy_evict_last();
+  // outlier rows are read once: evict them first, so that the score rows the atomics add into (just cleared) stay in L2
+  const uint64_t pol_keep = policy_evict_last(), pol_stream = policy_evict_first();
   for (uint32_t base = blockIdx.x * kOutPersThreads + (tid & ~31); base < total; base += stride) {
     const uint32_t e = base + lane;
     float contrib = 0.f;
@@ -608,11 +626,11 @@ __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
       int col;
       if constexpr (PAGED) {
         const int64_t pe = ((int64_t)page_of(pg, blockIdx.y, (int)t) * pg.P + t % (uint32_t)pg.P) * n_out + (e - t * (uint32_t)n_out);
-        v = outliers[pe];
-        col = outlier_idx[pe];
+        v = __uint_as_float(ld_stream_u32(reinterpret_cast<const uint32_t*>(outliers + pe), pol_stream));
+        col = (int)ld_stream_u32(reinterpret_cast<const uint32_t*>(outlier_idx + pe), pol_stream);
       } else {
-        v = outliers[e];
-        col = outlier_idx[e];
+        v = __uint_as_float(ld_stream_u32(reinterpret_cast<const uint32_t*>(outliers + e), pol_stream));
+        col = (int)ld_stream_u32(reinterpret_cast<const uint32_t*>(outlier_idx + e), pol_stream);
       }
       h = col >> 7;
       const int c = col & (kHeadDim - 1);
@@ -620,13 +638,15 @@ __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
       if (v != 0.f) {   // pads / non-outliers contribute exactly 0 in the reference too
         float2 cs;
         if (rope_theta > 0.f) {
-          // long contexts: the rope table no longer fits L2 and a scattered 8-byte gather costs a 32-byte DRAM sector
-          // (1M tokens: 17x the 128K cost for 8x the tokens) -- evaluate the table builder's own expressions instead
-          // (same device functions, same arguments: bit-identical values)
-          const int headdim = kHeadDim, headdim2 = headdim / 2;
-          const float th = powf(rope_theta, (-2 * __int2float_rd((c & (kHalf - 1)) % headdim2) / __int2float_rd(headdim)));
-          const int pos = (int)t + pos_offset;
-          cs = make_float2(cosf(th * pos), sinf(th * pos));
+          // the table builder's own expressions (same device functions, same arguments: bit-identical values) cost
+          // less than a scattered 8-byte gather, which past L2-sized tables is a 32-byte DRAM sector.  Past
+          // CUDART_TRIG_PLOSS_F, cosf / sinf leave their fast argument reduction for a local-memory one that stalls
+          // the whole warp; those arguments (rows j < 2 at 128K, j < 16 at 1M) come from the table, whose few rows
+          // stay in L2.
+          const int j = c & (kHalf - 1), pos = (int)t + pos_offset;
+          const float th = s_th[j];
+          if (th * pos <= CUDART_TRIG_PLOSS_F) cs = rope_cos_sin(th, pos);
+          else cs = ld_keep_f2(rope + (int64_t)j * rope_npos + pos, pol_keep);
         } else if (rope_h != nullptr) {   // fp16 mode: the half2 table the dense kernel streams (half the bytes per gather)
           uint32_t u;
           asm volatile("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(u)
@@ -683,12 +703,15 @@ static int k_out_impl_table() {   // KVQ_KOUT_IMPL=table selects the non-persist
   return v;
 }
 
-// rope tables beyond this many positions are not gathered from by the outlier scatter (KVQ_KOUT_DIRECT_NPOS overrides):
-// 64 pairs x 8 bytes x 64K positions = 32 MB, about what stays resident in the 50 MB L2 next to the streams
-static bool k_out_direct(int64_t n_positions) {
-  static int64_t thr = -1;
-  if (thr < 0) { const char* e = getenv("KVQ_KOUT_DIRECT_NPOS"); thr = e ? atoll(e) : 64 * 1024; }
-  return n_positions > thr;
+// Whether the outlier scatter computes its rotary factors (rope_row_theta / rope_cos_sin, bit-identical to the table)
+// instead of gathering them from the rope table.  Exact mode: at every length (one layer of 7B at 3 bits on an H100:
+// 15.4 against 20.0 us at 32K, DESIGN.md section 5).  fp16 mode (half_table): its half2 gather up to 64K positions
+// (64 pairs x 8 bytes x 64K = 32 MB of fp32 table, about what stays in the 50 MB L2 next to the streams), the exact
+// factors beyond.  KVQ_KOUT_DIRECT_NPOS=N overrides both: compute beyond N positions, gather up to N.
+static bool k_out_direct(int64_t n_positions, bool half_table) {
+  static int64_t thr = -2;
+  if (thr == -2) { const char* e = getenv("KVQ_KOUT_DIRECT_NPOS"); thr = e ? atoll(e) : -1; }
+  return n_positions > (thr >= 0 ? thr : (half_table ? 64 * 1024 : 0));
 }
 
 static int set_k_outlier_smem(size_t smem, bool gqa, bool batch, bool paged) {
@@ -736,16 +759,16 @@ static int launch_k_outliers(const KParams& p, int zero_first, float scale, cuda
     KVQ_LAUNCH_CHECK();
     return 0;
   }
-  const int rc = set_k_outlier_smem(smem, gqa, false, false);
+  const int rc = set_k_outlier_smem(smem + kOutThetaBytes, gqa, false, false);
   if (rc != 0) return rc;
   const unsigned grid = k_outlier_grid(total, smem, 1);
   // token-major target (fused path): a token's heads share one 128-byte line, so a warp's ~25 reductions (one or
   // two tokens) coalesce into one or two L1 requests instead of one per head row
   float* dst = p.opart != nullptr ? const_cast<float*>(p.opart) : p.out;
   const int64_t sh = p.opart != nullptr ? 1 : p.out_stride, stt = p.opart != nullptr ? p.opart_stride : 1;
-  const float direct_theta = k_out_direct(p.L + p.pos_offset) ? p.theta : 0.f;
+  const float direct_theta = k_out_direct(p.L + p.pos_offset, p.rope_h != nullptr) ? p.theta : 0.f;
   with_flavour(gqa, false, false, [&](auto GQA, auto BATCH, auto PAGED) {
-    k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem, st>>>(
+    k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, st>>>(
         p.q, p.outliers, p.outlier_idx, dst, sh, stt, p.L, p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset, scale,
         p.len_dev, p.len_add, p.rope_h, direct_theta, gqa ? p.grp : 1, 0, 0, PageRef{});
   });
@@ -753,18 +776,12 @@ static int launch_k_outliers(const KParams& p, int zero_first, float scale, cuda
   return 0;
 }
 
-// rope table: reference expressions quant_cuda_kernel.cu:3081 (theta) and 3123-3126 (cos/sin), once per (j, p)
+// rope table: rope_row_theta / rope_cos_sin once per (j, p)
 __global__ void rope_table_kernel(float2* __restrict__ out, float rope_theta, int64_t n_pos) {
   const int j = blockIdx.y;
-  const int headdim = kHeadDim;
-  const int headdim2 = headdim / 2;
-  const float theta = powf(rope_theta, (-2 * __int2float_rd(j % headdim2) / __int2float_rd(headdim)));
-  for (int64_t pos64 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos64 < n_pos; pos64 += (int64_t)gridDim.x * blockDim.x) {
-    const int pos = (int)pos64;
-    const float c = cosf(theta * pos);
-    const float s = sinf(theta * pos);
-    out[(int64_t)j * n_pos + pos64] = make_float2(c, s);
-  }
+  const float theta = rope_row_theta(rope_theta, j);
+  for (int64_t pos64 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos64 < n_pos; pos64 += (int64_t)gridDim.x * blockDim.x)
+    out[(int64_t)j * n_pos + pos64] = rope_cos_sin(theta, (int)pos64);
 }
 
 template <int BITS>
@@ -915,13 +932,13 @@ int k_scores_batch(const AttendCall& c, const AttendScratch& s) {
     k_batch_zero_kernel<<<dim3((unsigned)std::min<int64_t>((c.L + 2047) / 2048, 64), H, B), 256, 0, c.stream>>>(
         s.scores, s.stride, s.bstride, c.len_dev, c.len_add, c.L);
     KVQ_LAUNCH_CHECK();
-    const int rc = set_k_outlier_smem(smem, grp > 1, true, c.pg != nullptr);
+    const int rc = set_k_outlier_smem(smem + kOutThetaBytes, grp > 1, true, c.pg != nullptr);
     if (rc != 0) return rc;
     const dim3 grid(k_outlier_grid(c.L * c.n_out, smem, B), (unsigned)B);
-    const float direct_theta = k_out_direct(c.L + c.pos_offset) ? c.theta : 0.f;
+    const float direct_theta = k_out_direct(c.L + c.pos_offset, false) ? c.theta : 0.f;
     const int64_t b_rows = c.pg != nullptr ? 0 : c.Lmax * c.n_out;   // a pool has no per-sequence row block
     with_flavour(grp > 1, true, c.pg != nullptr, [&](auto GQA, auto BATCH, auto PAGED) {
-      k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem, c.stream>>>(
+      k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
           c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, reinterpret_cast<const float2*>(c.rope),
           c.rope_npos, c.pos_offset, 1.f, c.len_dev, c.len_add, nullptr, direct_theta, grp, s.bstride, b_rows,
           c.pg != nullptr ? *c.pg : PageRef{});
