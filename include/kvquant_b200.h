@@ -180,9 +180,9 @@ KVQ_API int kvq_attend_dyn(int bits, const float* q, const int32_t* kcache, cons
  *   Shapes: Hq <= 64, Hq % 4 == 0, Hkv % 4 == 0, Hq % Hkv == 0; anything else is KVQ_E_SHAPE.
  *   kvq_attend_gqa / kvq_attend_gqa_dyn: kvq_attend / kvq_attend_dyn with (Hq, Hkv) in place of H; scratch of
  *   kvq_attend_scratch_bytes(Hq, L) (or L_cap) bytes.  With Hq == Hkv they are kvq_attend / kvq_attend_dyn.  With
- *   g > 1: native V form (v_cent + v_aff) and exact tables only -- a missing v_cent / v_aff, a non-NULL rope_half or
- *   a set KVQ_K_IMPL return KVQ_E_UNSUPPORTED.  Each KV head's packed words and outlier rows are read once per token
- *   range and serve its g query heads.
+ *   g > 1: native V form (v_cent + v_aff) and exact tables only -- a missing v_cent / v_aff or a non-NULL rope_half
+ *   return KVQ_E_UNSUPPORTED.  Each KV head's packed words and outlier rows are read once per token range and serve
+ *   its g query heads.
  *   kvq_attend_chunk_gqa: kvq_attend_chunk with q / out [T, Hq, 128], chunk_k / chunk_v f16 [Hkv, T, 128]; scratch of
  *   kvq_attend_chunk_scratch_bytes(Hq, T, L) bytes.
  *   kvq_dec_rope_split_gqa[_dyn]: qkv fp16 [(Hq + 2*Hkv)*128] = q | k | v -> q f32 [Hq*128] (rotated as
@@ -218,7 +218,7 @@ KVQ_API int kvq_attend_gqa_dyn(int bits, const float* q, const int32_t* kcache, 
  *     no active mask: with len_add > 0 a sequence that did not append this step attends a slot it never wrote, and
  *     its output is meaningless (the caller ignores it).  Shapes of
  *     kvq_attend_gqa (Hq == Hkv included) and 1 <= B <= 256, else KVQ_E_SHAPE; exact fp32 tables and the native V
- *     form only (a missing v_cent / v_aff, a non-NULL rope_half or a set KVQ_K_IMPL return KVQ_E_UNSUPPORTED).  A
+ *     form only (a missing v_cent / v_aff or a non-NULL rope_half return KVQ_E_UNSUPPORTED).  A
  *     sequence with no slot and no sink (an idle serving slot) writes out = 0 and lse = -inf.  The split counts are
  *     sized so that B x splits x head groups fill the SMs.  scratch: kvq_attend_batch_scratch_bytes(B, Hq, L_cap)
  *     bytes, 16-byte aligned (B blocks of kvq_attend_scratch_bytes(Hq, L_cap): sequence b's tables, scores,

@@ -6,7 +6,6 @@
 //   attend_init -> K outliers + dense K scores (kvq_kscore.cu) -> softmax . V partials (kvq_vnative.cu) -> attend_combine
 // over a scratch laid out by attend_scratch().  This file holds the init / combine / merge kernels and that host side.
 #include "kvq_attend.cuh"
-#include <stdlib.h>
 #include <cuda_fp16.h>
 
 namespace kvq {
@@ -134,24 +133,15 @@ AttendScratch attend_scratch(void* scratch, int H, int64_t L, int bits) {
   int64_t off = 0;   // floats; every block below is a multiple of 4 floats (H % 4 == 0), so each starts 16-byte aligned
   auto take = [&](int64_t n) { float* p = base ? base + off : nullptr; off += n; return p; };
   s.stride = round_up(L, 32);
-  s.opart_stride = (int)round_up(H, 32);
   s.scores = take(H * s.stride);
   s.gmax = take(H);
   s.sink_scores = take((int64_t)H * 64);
   s.part_o = take((int64_t)kMaxPart * H * kHeadDim);
   s.part_l = take((int64_t)kMaxPart * H);
-  s.opart = take(s.stride * s.opart_stride);
   s.qtab = take((int64_t)H * kHeadDim * 17);   // sized for 4 bits: 16 table entries and one ratio per channel
   s.qrat = base ? s.qtab + (int64_t)H * kHeadDim * (1 << bits) : nullptr;
   s.bstride = off + 64;
   return s;
-}
-
-// KVQ_K_IMPL set (generic / pair / kappa / lds64): round 1's 8-byte-entry kernels serve the exact mode of the fused attend
-static int k_legacy_fused() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("KVQ_K_IMPL"); v = (e && e[0]) ? 1 : 0; }
-  return v;
 }
 
 // Grouped-query attention: Hq query heads over an Hkv-head cache, query head h attending over KV head h / (Hq / Hkv).
@@ -161,7 +151,7 @@ static int check_gqa(int Hq, int Hkv) {
   return 0;
 }
 static int gqa_unsupported(const AttendCall& c) {
-  return (c.v_cent == nullptr || c.v_aff == nullptr || c.rope_half != nullptr || k_legacy_fused()) ? KVQ_E_UNSUPPORTED : 0;
+  return (c.v_cent == nullptr || c.v_aff == nullptr || c.rope_half != nullptr) ? KVQ_E_UNSUPPORTED : 0;
 }
 // the preconditions of kvq_attend_gqa[_dyn] and kvq_attend_dyn, checked ahead of attend_validate
 static int check_gqa_call(const AttendCall& c) {
@@ -226,10 +216,7 @@ static int attend_run(const AttendCall& c) {
   KVQ_LAUNCH_CHECK();
   int n_cta = 0;
   if (batch || c.L > 0) {
-    // one sequence: KVQ_K_IMPL (generic / pair / kappa) keeps round 1's LDS.64 kernels reachable for A/B runs;
-    // otherwise the TMA-fed kernels: exact fp32 ratio form, or (rope_half given) the fp16-table form
-    int rc = batch ? k_scores_batch(c, s)
-           : (c.rope_half == nullptr && k_legacy_fused()) ? k_scores_fused(c, s) : k_scores_fused_fast(c, s);
+    int rc = batch ? k_scores_batch(c, s) : k_scores_fused(c, s);
     if (rc) return rc;
     rc = (c.v_cent != nullptr && c.v_aff != nullptr) ? v_native_dispatch(c, s, &n_cta) : v_accum_fused(c, s, &n_cta);
     if (rc) return rc;

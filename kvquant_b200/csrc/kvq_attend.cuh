@@ -60,26 +60,22 @@ struct AttendScratch {
   float* sink_scores;   // [Hq][64]
   float* part_o;        // [kMaxPart][Hq][128]
   float* part_l;        // [kMaxPart][Hq]
-  float* opart;         // token-major K-outlier partials [stride][opart_stride]
   float* qtab;          // premultiplied K table [Hq][128][2^bits] ...
   float* qrat;          // ... and ratios [Hq][128] of the exact K form
   int64_t stride;       // L rounded up to 32
-  int opart_stride;     // Hq rounded up to 32: one 128-byte line per 32 heads
   int64_t bstride;      // floats per sequence block (a multiple of 4)
 };
 // the layout for Hq heads and L tokens over `scratch` (null: sizes only); every block starts 16-byte aligned
 AttendScratch attend_scratch(void* scratch, int H, int64_t L, int bits);
 
-// K side.  k_scores_fused: the LDS.64 kernels kept behind KVQ_K_IMPL; k_scores_fused_fast: outlier scatter + the
-// TMA-fed dense kernel (exact ratio form, or the fp16-table form when c.rope_half is set); k_scores_batch: the same
-// for a (paged) batch, exact form only.  All in kvq_kscore.cu.
+// K side.  k_scores_fused: outlier scatter + the TMA-fed dense kernel (exact ratio form, or the fp16-table form when
+// c.rope_half is set); k_scores_batch: the same for a (paged) batch, exact form only.  Both in kvq_kscore.cu.
 int k_scores_fused(const AttendCall& c, const AttendScratch& s);
-int k_scores_fused_fast(const AttendCall& c, const AttendScratch& s);
 int k_scores_batch(const AttendCall& c, const AttendScratch& s);
-// dense K kernels over tokens [t0, t0 + Lb) (KVQ_K_BLOCK walks a long cache in blocks): kvq_kratio.cu, kvq_kfast.cu.
+// dense K kernels over tokens [0, c.L): kvq_kratio.cu, kvq_kfast.cu.
 // accumulate != 0: s.scores holds the unscaled outlier partial sums on entry.
-int k_ratio_dispatch(const AttendCall& c, const AttendScratch& s, int64_t t0, int64_t Lb, int run_prep, int accumulate);
-int k_fast_dispatch(const AttendCall& c, const AttendScratch& s, int64_t t0, int64_t Lb, int run_prep, int accumulate);
+int k_ratio_dispatch(const AttendCall& c, const AttendScratch& s, int accumulate);
+int k_fast_dispatch(const AttendCall& c, const AttendScratch& s, int accumulate);
 // V side: softmax weights from s.scores / s.gmax, partial rows into s.part_o / s.part_l, their count in *n_cta.
 // Native form (kvq_vnative.cu) and the form over materialised LUT rows (kvq_vaccum.cu).
 int v_native_dispatch(const AttendCall& c, const AttendScratch& s, int* n_cta);

@@ -3,11 +3,10 @@
 // Replaces (reference deployment/kvquant/quant_cuda_kernel.cu):
 //   VecQuant3MatMulKernelNUQPerChannelTransposedRopeMHABatchedFusedOpt   3692-4115
 //
-// Same arithmetic as k_scores_kernel<3> (kvq_kscore.cu): T[h][c][code] = (LUT q_c, s_c LUT q_c^64), one LDS.64 +
-// two FFMA per element.  What differs is how the 96-bit code streams are fed:
+// The arithmetic of k_scores_kernel (kvq_kscore.cu, 4 and 2 bits): T[h][c][code] = (LUT q_c, s_c LUT q_c^64), one
+// LDS.64 + two FFMA per element.  The 96-bit code streams are fed so that:
 //   * every packed word is loaded exactly ONCE: the four 24-bit windows of a 32-channel group are funnel-shifted out
-//     of the current and the carried word (the generic kernel loads both words of every window: 8 loads per 3
-//     words);
+//     of the current and the carried word;
 //   * G = 8 heads per CTA (64 KiB of tables) -> H/8 head groups x (SMs / groups) token ranges, one CTA per SM;
 //   * token ranges are cut at warp granularity and a warp whose 32 tokens lie past the range skips the tile, so the
 //     last tile of a range costs only its live warps.
@@ -56,10 +55,8 @@ __global__ void __launch_bounds__(K3Cfg::kThreads, 1) k_scores3_kernel(const KPa
   const uint32_t tab0 = smem_u32(s_tab);
 
   // this CTA's token range [t_begin, t_limit): p.range is a multiple of 32
-  const int64_t L_eff = k_eff_len(p);
-  const int64_t range = k_eff_range(p, L_eff);
-  const int64_t t_begin = (int64_t)blockIdx.x * range;
-  const int64_t t_limit = min(L_eff, t_begin + range);
+  const int64_t t_begin = (int64_t)blockIdx.x * p.range;
+  const int64_t t_limit = min(p.L, t_begin + p.range);
   if (t_begin >= t_limit) return;
   const uint32_t pitch = (uint32_t)p.Lmax * 4u;
   const unsigned char* cb0 = reinterpret_cast<const unsigned char*>(p.cache + (int64_t)h0 * W * p.Lmax);
@@ -141,27 +138,11 @@ __global__ void __launch_bounds__(K3Cfg::kThreads, 1) k_scores3_kernel(const KPa
         });
       }
 
-      float old[G];
 #pragma unroll
       for (int hl = 0; hl < G; ++hl) {
-        old[hl] = 0.f;
-        if (p.accumulate && live && (FULL || hl < nh)) old[hl] = p.out[(int64_t)(h0 + hl) * p.out_stride + t];
-      }
-      if (p.opart != nullptr && live) {   // outlier partials of this token's 8 heads: two 16-byte loads (rows are padded)
-        const float4* src = reinterpret_cast<const float4*>(p.opart + t * p.opart_stride + h0);
-        const float4 a = __ldcg(src), b = __ldcg(src + 1);
-        old[0] += a.x; old[1] += a.y; old[2] += a.z; old[3] += a.w;
-        old[4] += b.x; old[5] += b.y; old[6] += b.z; old[7] += b.w;
-      }
-#pragma unroll
-      for (int hl = 0; hl < G; ++hl) {
-        if (FULL || hl < nh) {
-          const float s = ((acc[hl].x + acc[hl].y) + old[hl]) * p.scale;
-          if (live) p.out[(int64_t)(h0 + hl) * p.out_stride + t] = s;
-          if (p.gmax != nullptr) {
-            const float m = warp_max(live ? s : -INFINITY);
-            if ((tid & 31) == 0 && m > -INFINITY) atomic_max_float(p.gmax + h0 + hl, m);
-          }
+        if (live && (FULL || hl < nh)) {
+          float* o = p.out + (int64_t)(h0 + hl) * p.out_stride + t;
+          *o = (acc[hl].x + acc[hl].y) + *o;
         }
       }
     }
@@ -182,9 +163,7 @@ int k_scores3_dispatch(const KParams& p, cudaStream_t st) {
     attr_done = true;
   }
   const int n_groups = (p.H + C::G - 1) / C::G;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms_cached();
   const int64_t max_splits = sms / n_groups > 0 ? sms / n_groups : 1;
   KParams q = p;
   q.range = k_token_range(p.L, max_splits);

@@ -44,7 +44,6 @@ struct KRParams {
   float* out;                // [H][out_stride]
   float* gmax;               // [H] or null
   int64_t Lmax, L, out_stride, rope_npos, range;
-  int64_t t0;                // first token of this launch (long caches are walked in L2-sized blocks)
   const int64_t* len_dev;
   int64_t len_add;
   int H, G, pos_offset, accumulate, n_stages;   // H, G: query heads (of the call, of one CTA)
@@ -215,7 +214,7 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
   int64_t L_eff = p.L;
   int64_t range = p.range;
   if (p.len_dev != nullptr) {
-    const int64_t l = p.len_dev[bz] + p.len_add - p.t0;
+    const int64_t l = p.len_dev[bz] + p.len_add;
     L_eff = l < 0 ? 0 : (l < p.L ? l : p.L);
     if constexpr (PAGED) {
       const int64_t cap = page_cap(pg, bz);
@@ -226,8 +225,8 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
       range = kr_range(L_eff, gridDim.x);
     }
   }
-  const int64_t t_begin = p.t0 + (int64_t)blockIdx.x * range;
-  const int64_t t_limit = p.t0 + min(L_eff, ((int64_t)blockIdx.x + 1) * range);
+  const int64_t t_begin = (int64_t)blockIdx.x * range;
+  const int64_t t_limit = min(L_eff, ((int64_t)blockIdx.x + 1) * range);
   if (t_begin >= t_limit) return;
   const int ncols = (int)((t_limit - t_begin + kKRColTok - 1) / kKRColTok);
   const int nrounds = (ncols + kKRWarps - 1) / kKRWarps;
@@ -391,18 +390,16 @@ static int set_k_ratio_smem() {
 // c.B == 0: one sequence; c.B >= 1: a batch of B sequences, each with its own scratch block of s.bstride floats;
 // c.pg != nullptr: a paged batch (the grid is the contiguous batch's)
 template <int BITS>
-static int launch_k_ratio(KRParams p, const AttendCall& c, const AttendScratch& s, int run_prep) {
+static int launch_k_ratio(KRParams p, const AttendCall& c, const AttendScratch& s) {
   using C = KRCfg<BITS>;
   const int B = c.B, grp = c.grp();
   const bool gqa = grp > 1, batch = B > 0, paged = c.pg != nullptr;
   cudaStream_t st = c.stream;
-  if (run_prep) {
-    with_flavour(gqa, batch, false, [&](auto GQA, auto BATCH, auto) {
-      k_ratio_prep_kernel<BITS, GQA(), BATCH()><<<batch ? dim3(p.H, B) : dim3(p.H), kHeadDim, 0, st>>>(
-          c.q, c.klut, s.qtab, s.qrat, grp, s.bstride);
-    });
-    KVQ_LAUNCH_CHECK();
-  }
+  with_flavour(gqa, batch, false, [&](auto GQA, auto BATCH, auto) {
+    k_ratio_prep_kernel<BITS, GQA(), BATCH()><<<batch ? dim3(p.H, B) : dim3(p.H), kHeadDim, 0, st>>>(
+        c.q, c.klut, s.qtab, s.qrat, grp, s.bstride);
+  });
+  KVQ_LAUNCH_CHECK();
   // CTA head groups of at most GMAX query heads; under GQA whole KV-head groups (grp <= 16 <= GMAX)
   const int Hkv = p.H / grp, kv_max = C::GMAX / grp;
   const int groups = (Hkv + kv_max - 1) / kv_max;
@@ -442,20 +439,20 @@ static int launch_k_ratio(KRParams p, const AttendCall& c, const AttendScratch& 
   return 0;
 }
 
-// dense K scores of the fused attend, fp32 ratio form, tokens [t0, t0 + Lb).  s.scores holds the (unscaled) outlier
-// partial sums on entry when accumulate != 0.  s.qtab / s.qrat: Hq * 128 * (2^bits + 1) floats of scratch.
-int k_ratio_dispatch(const AttendCall& c, const AttendScratch& s, int64_t t0, int64_t Lb, int run_prep, int accumulate) {
+// dense K scores of the fused attend, fp32 ratio form.  s.scores holds the (unscaled) outlier partial sums on entry
+// when accumulate != 0.  s.qtab / s.qrat: Hq * 128 * (2^bits + 1) floats of scratch.
+int k_ratio_dispatch(const AttendCall& c, const AttendScratch& s, int accumulate) {
   KRParams p{};
   p.qtab = s.qtab; p.qrat = s.qrat;
   p.rope = reinterpret_cast<const float2*>(c.rope);
   p.out = s.scores; p.gmax = s.gmax;
-  p.Lmax = c.Lmax; p.L = Lb; p.out_stride = s.stride; p.rope_npos = c.rope_npos;
-  p.len_dev = c.len_dev; p.len_add = c.len_add; p.t0 = t0;
+  p.Lmax = c.Lmax; p.L = c.L; p.out_stride = s.stride; p.rope_npos = c.rope_npos;
+  p.len_dev = c.len_dev; p.len_add = c.len_add;
   p.H = c.Hq; p.pos_offset = c.pos_offset; p.accumulate = accumulate; p.scale = kAttendScale;
   switch (c.bits) {
-    case 4: return launch_k_ratio<4>(p, c, s, run_prep);
-    case 3: return launch_k_ratio<3>(p, c, s, run_prep);
-    case 2: return launch_k_ratio<2>(p, c, s, run_prep);
+    case 4: return launch_k_ratio<4>(p, c, s);
+    case 3: return launch_k_ratio<3>(p, c, s);
+    case 2: return launch_k_ratio<2>(p, c, s);
     default: return KVQ_E_BITS;
   }
 }

@@ -131,13 +131,13 @@ def test_first_failed_check_decides_the_code():
 
 def _scratch_bytes(H, L):
     """The layout of one sequence's scratch, in floats: score rows, per-head max, sink scores, 256 partial (o, l)
-    rows, token-major outlier partials, the 4-bit K table with its ratios; 256 bytes of slack."""
+    rows, the 4-bit K table with its ratios; 256 bytes of slack."""
     r32 = lambda x: (x + 31) // 32 * 32     # noqa: E731
-    floats = H * r32(L) + H + H * 64 + 256 * H * 128 + 256 * H + r32(L) * r32(H) + H * 128 * 17
+    floats = H * r32(L) + H + H * 64 + 256 * H * 128 + 256 * H + H * 128 * 17
     return 4 * floats + 256
 
 
-def test_scratch_bytes_formula():
+def test_scratch_bytes_closed_form():
     lib = _lib.load()
     for H in range(4, 65, 4):
         for L in (1, 31, 32, 33, 200, 1000, 4096, 32768, 131072, 1 << 20):
