@@ -86,6 +86,16 @@ KVQ_API int kvq_append_v_sparse_parallel(int bits, int32_t* cache, const float* 
 KVQ_API int kvq_rope_table_build(float* rope_cos_sin, float theta, int64_t n_pos, void* stream);
 /* The same table rounded once to fp16: half2 [64, n_pos] = (cos, sin) -- read by the fp16 mode of kvq_attend. */
 KVQ_API int kvq_rope_table_build_half(void* rope_half, float theta, int64_t n_pos, void* stream);
+/* Scaled rotary frequencies (HF rope_type "linear", "llama3", "yarn"; DESIGN.md section 4.13): the same layouts built
+ * from a frequency vector instead of theta,
+ *   rope[j*n_pos + p] = (cosf(freq[j]*p) * attn_factor, sinf(freq[j]*p) * attn_factor),  j < 64,
+ * freq = f32 [64] DEVICE pointer (HF's inv_freq; read on the stream, so the build can be captured), attn_factor = HF's
+ * attention_factor (1 except for YaRN), finite and > 0.  With attn_factor == 1 each entry is exactly cosf / sinf of
+ * freq[j]*p.  NULL pointers -> KVQ_E_NULL; n_pos outside [1, 2^30] or a bad attn_factor -> KVQ_E_SHAPE. */
+KVQ_API int kvq_rope_table_build_freq(float* rope_cos_sin, const float* freq, float attn_factor, int64_t n_pos,
+                                      void* stream);
+KVQ_API int kvq_rope_table_build_freq_half(void* rope_half, const float* freq, float attn_factor, int64_t n_pos,
+                                           void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Legacy decode matvecs (results are ADDED to `mul`, which the caller pre-zeroes -- modeling_llama.py:782,1209).
@@ -205,6 +215,32 @@ KVQ_API int kvq_attend_gqa_dyn(int bits, const float* q, const int32_t* kcache, 
                    float* out, float* out_lse, void* scratch, const void* rope_half, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Scaled rotary frequencies (DESIGN.md section 4.13): kvq_attend_gqa, kvq_attend_gqa_dyn, kvq_attend_batch and
+ * kvq_attend_paged with (const float* rope_freq, float attn_factor) in place of `float theta`.  rope_cos_sin (and
+ * rope_half) must be the tables kvq_rope_table_build_freq[_half] built from the same rope_freq (f32 [64], device) and
+ * attn_factor; the K outlier pass computes its factors from rope_freq and attn_factor with the table builder's
+ * expressions, bit for bit the table's entries.  The cache itself (pre-RoPE keys) is the same for every frequency
+ * vector.  Argument checks: the parent's, in the parent's order, with the parent's codes; then rope_freq == NULL ->
+ * KVQ_E_NULL and attn_factor not finite or <= 0 -> KVQ_E_SHAPE.
+ * ------------------------------------------------------------------------------------------------------------- */
+KVQ_API int kvq_attend_gqa_freq(int bits, const float* q,
+                   const int32_t* kcache, const float* klut,
+                   const float* k_outliers, const int32_t* k_outlier_idx,
+                   const int32_t* vcache, const float* vlut_tok, const float* v_cent, const float* v_aff,
+                   const float* v_outliers, const int32_t* v_outlier_idx,
+                   int n_out, int Hq, int Hkv, int64_t Lmax, int64_t L,
+                   const float* rope_cos_sin, int64_t rope_npos, const float* rope_freq, float attn_factor,
+                   int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
+                   float* out, float* out_lse, void* scratch, const void* rope_half, void* stream);
+KVQ_API int kvq_attend_gqa_dyn_freq(int bits, const float* q, const int32_t* kcache, const float* klut,
+                   const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent,
+                   const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv,
+                   int64_t Lmax, int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
+                   int64_t rope_npos, const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                   const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch, const void* rope_half,
+                   void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Batched decode: B sequences of one layer in one launch set.  The layer's cache for B sequences is batch-strided, and
  * sequence b's slice of every tensor has exactly the layout of a single-sequence cache (Lmax % 4 == 0 keeps each
  * slice 16-byte aligned): kcache / vcache int32 [B, Hkv, W, Lmax]; outlier values f32 and indices int32 [B, Lmax, n_out];
@@ -288,6 +324,21 @@ KVQ_API int kvq_attend_paged(int bits, int B, const float* q, const int32_t* kca
                    int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
                    float* out, float* out_lse, void* scratch, const void* rope_half, void* stream,
                    const int32_t* page_table, int max_pages, const int32_t* npages, int P);
+/* kvq_attend_batch / kvq_attend_paged over tables built from a frequency vector (see kvq_attend_gqa_freq) */
+KVQ_API int kvq_attend_batch_freq(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                   const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent,
+                   const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv,
+                   int64_t Lmax, int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
+                   int64_t rope_npos, const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                   const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch, const void* rope_half,
+                   void* stream);
+KVQ_API int kvq_attend_paged_freq(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                   const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent,
+                   const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv,
+                   int n_pool, int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
+                   int64_t rope_npos, const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                   const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch, const void* rope_half,
+                   void* stream, const int32_t* page_table, int max_pages, const int32_t* npages, int P);
 KVQ_API int kvq_page_copy(int bits, int H, int n_out, int P, int64_t s0, int64_t s1, const kvq_seq_ref* src,
                           const kvq_seq_ref* dst, void* stream);
 
@@ -495,6 +546,14 @@ KVQ_API int kvq_dec_rope_split_gqa_dyn(const void* qkv_f16, const float* inv_fre
 KVQ_API int kvq_dec_counter_add(int64_t* counter, int64_t delta, void* stream);
 KVQ_API int kvq_dec_rope_split_batch(const void* qkv_f16, const float* inv_freq, const int64_t* pos_dev, int64_t pos_add,
                                      float* q, float* k, float* v, int Hq, int Hkv, int B, void* stream);
+/* Query rotation for scaled rotary frequencies: qkv fp16 [B, (Hq + 2*Hkv)*128] -> q f32 [B, Hq*128], row b rotated at
+ * pos_add (+ pos_dev[b] when pos_dev is not NULL) with cos / sin of inv_freq[j]*pos each multiplied by attn_factor (HF
+ * applies YaRN's attention_factor to queries and keys alike); k, v f32 [B, Hkv*128].  With attn_factor == 1 a row is
+ * exactly what kvq_dec_rope_split_gqa[_dyn] / kvq_dec_rope_split_batch compute.  attn_factor not finite or <= 0, or
+ * B outside [1, 65535] -> KVQ_E_SHAPE. */
+KVQ_API int kvq_dec_rope_split_freq(const void* qkv_f16, const float* inv_freq, float attn_factor,
+                                    const int64_t* pos_dev, int64_t pos_add, float* q, float* k, float* v, int Hq,
+                                    int Hkv, int B, void* stream);
 KVQ_API int kvq_dec_counter_add_batch(int64_t* counter, const int32_t* active, int64_t delta, int B, void* stream);
 KVQ_API int kvq_dec_silu_mul(const void* gu_f16, void* act_f16, int n, void* stream);
 KVQ_API int kvq_dec_f32_to_f16(const float* a, void* b_f16, int n, void* stream);

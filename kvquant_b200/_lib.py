@@ -28,6 +28,8 @@ SIGNATURES = {
     "kvq_append_v_sparse_parallel": (_c_int, [_c_int, _p, _p, _p, _p, _p, _c_int, _c_i64, _c_i64, _p]),
     "kvq_rope_table_build": (_c_int, [_p, _c_f, _c_i64, _p]),
     "kvq_rope_table_build_half": (_c_int, [_p, _c_f, _c_i64, _p]),
+    "kvq_rope_table_build_freq": (_c_int, [_p, _p, _c_f, _c_i64, _p]),
+    "kvq_rope_table_build_freq_half": (_c_int, [_p, _p, _c_f, _c_i64, _p]),
     "kvq_k_matvec": (_c_int, [_c_int, _p, _p, _p, _p, _c_int, _c_int, _c_i64, _c_i64, _p, _p, _c_int, _p, _c_i64,
                               _c_f, _c_int, _p]),
     "kvq_v_matvec": (_c_int, [_c_int, _p, _p, _p, _p, _c_int, _c_int, _c_i64, _c_i64, _p, _p, _c_int, _p]),
@@ -38,6 +40,11 @@ SIGNATURES = {
                                 _c_i64, _p, _c_i64, _c_f, _c_int, _p, _p, _c_int, _p, _p, _p, _p, _p]),
     "kvq_attend_gqa_dyn": (_c_int, [_c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int, _c_int, _c_i64,
                                     _c_i64, _p, _c_i64, _p, _c_i64, _c_f, _c_int, _p, _p, _c_int, _p, _p, _p, _p, _p]),
+    "kvq_attend_gqa_freq": (_c_int, [_c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int, _c_int,
+                                     _c_i64, _c_i64, _p, _c_i64, _p, _c_f, _c_int, _p, _p, _c_int, _p, _p, _p, _p, _p]),
+    "kvq_attend_gqa_dyn_freq": (_c_int, [_c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int, _c_int,
+                                         _c_i64, _c_i64, _p, _c_i64, _p, _c_i64, _p, _c_f, _c_int, _p, _p, _c_int, _p,
+                                         _p, _p, _p, _p]),
     "kvq_attend_merge": (_c_int, [_p, _c_int, _c_int, _p, _p]),
     "kvq_append_kv_fused_batch": (_c_int, [_c_int, _c_int, _c_int, _c_i64, _p, _c_i64, _p, _c_int, _p, _p, _p, _p, _p,
                                            _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
@@ -50,6 +57,12 @@ SIGNATURES = {
     "kvq_attend_paged": (_c_int, [_c_int, _c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int, _c_int,
                                   _c_int, _c_i64, _p, _c_i64, _p, _c_i64, _c_f, _c_int, _p, _p, _c_int, _p, _p, _p, _p,
                                   _p, _p, _c_int, _p, _c_int]),
+    "kvq_attend_batch_freq": (_c_int, [_c_int, _c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int,
+                                       _c_int, _c_i64, _c_i64, _p, _c_i64, _p, _c_i64, _p, _c_f, _c_int, _p, _p,
+                                       _c_int, _p, _p, _p, _p, _p]),
+    "kvq_attend_paged_freq": (_c_int, [_c_int, _c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int,
+                                       _c_int, _c_int, _c_i64, _p, _c_i64, _p, _c_i64, _p, _c_f, _c_int, _p, _p,
+                                       _c_int, _p, _p, _p, _p, _p, _p, _c_int, _p, _c_int]),
     "kvq_page_copy": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_i64, _c_i64, _p, _p, _p]),
     "kvq_append_kv_fused": (_c_int, [_c_int, _c_int, _c_i64, _c_i64, _c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                      _p, _p, _p, _p, _p, _p, _p]),
@@ -88,6 +101,7 @@ SIGNATURES = {
     "kvq_dec_rope_split_gqa_dyn": (_c_int, [_p, _p, _p, _c_i64, _p, _p, _p, _c_int, _c_int, _p]),
     "kvq_dec_counter_add": (_c_int, [_p, _c_i64, _p]),
     "kvq_dec_rope_split_batch": (_c_int, [_p, _p, _p, _c_i64, _p, _p, _p, _c_int, _c_int, _c_int, _p]),
+    "kvq_dec_rope_split_freq": (_c_int, [_p, _p, _c_f, _p, _c_i64, _p, _p, _p, _c_int, _c_int, _c_int, _p]),
     "kvq_dec_counter_add_batch": (_c_int, [_p, _p, _c_i64, _c_int, _p]),
     "kvq_dec_silu_mul": (_c_int, [_p, _p, _c_int, _p]),
     "kvq_dec_f32_to_f16": (_c_int, [_p, _p, _c_int, _p]),

@@ -19,6 +19,7 @@ import torch
 
 from . import _lib
 from . import quant_cuda as qc
+from .rope import RotarySpec, resolve as _resolve_rope
 
 HEAD_DIM = 128
 
@@ -46,6 +47,15 @@ def build_k_lookup_table(upper, lower, centroids, num_heads, normscale=None, nor
         c2 = cent * float(normscale) + float(normoffset)
         out["lut2"] = (c2[None, :] * sf + off).contiguous().view(num_heads, HEAD_DIM, -1)
     return out
+
+
+def _rope_call(device, rope):
+    """(entry point suffix, rotary arguments) of a fused attend over tables for `rope` (a float theta or a scaled
+    RotarySpec): the theta entry points take theta, their *_freq siblings the device frequency vector and the
+    attention factor in its place."""
+    if isinstance(rope, RotarySpec):
+        return "_freq", (qc.rope_freq(device, rope).data_ptr(), float(rope.attention_factor))
+    return "", (float(rope),)
 
 
 def _on_cache_device(fn):
@@ -280,18 +290,20 @@ class LayerCache:
         self.len += T
 
     @_on_cache_device
-    def attend(self, q, rope_theta=10000.0, out=None, lse=None):
+    def attend(self, q, rope_theta=10000.0, out=None, lse=None, rope=None):
         """softmax(q.K^T/sqrt(128)).V over sinks + quantised slots.  q: f32 [H,128] already rotated at its own
         position.  Returns f32 [H,128].  lse (optional f32 [H]) receives the log-sum-exp of the scaled scores, which
         lets partial results over disjoint token ranges be merged exactly (sequence-sharded decode).
-        Grouped-query cache: q, out f32 [q_heads, 128], lse [q_heads] (kvq_attend_gqa)."""
+        Grouped-query cache: q, out f32 [q_heads, 128], lse [q_heads] (kvq_attend_gqa).
+        rope (optional RotarySpec): the keys' rotary frequencies in place of rope_theta (scaled RoPE: the
+        kvq_attend_gqa_freq entry points); q must be rotated with the same spec."""
         if self.group > 1:
             self._gqa_check()
         elif self.v_norm is not None and not self.use_native_v:
             # the per-token LUT rows hold the un-normed centroids while the outlier residuals were taken against the
             # Q-Norm table: the legacy-LUT V kernel would mix the two
             raise NotImplementedError("V Q-Norm needs the native V form (use_native_v=True)")
-        return self._attend(q, None, 0, rope_theta, out, lse, self.len)
+        return self._attend(q, None, 0, _resolve_rope(rope, rope_theta), out, lse, self.len)
 
     def _attend(self, q, len_dev, len_add, rope_theta, out, lse, L):
         """attend over L slots (len_dev None: kvq_attend_gqa) or attend_dyn with the cap L (kvq_attend_gqa_dyn).  With
@@ -307,16 +319,18 @@ class LayerCache:
                 *self._out_ptrs("k"), self.vcache.data_ptr())
         vpart = (self.v_cent_deq.data_ptr() if native else None, self.vaff.data_ptr() if native else None,
                  *self._out_ptrs("v"), self.n_out, self.Hq, self.H, self.Lmax, L)
-        tail = (rope.data_ptr(), npos, float(rope_theta), pos_offset, self.sink_k.data_ptr() if ns else None,
+        sfx, rargs = _rope_call(self.device, rope_theta)
+        tail = (rope.data_ptr(), npos, *rargs, pos_offset, self.sink_k.data_ptr() if ns else None,
                 self.sink_v.data_ptr() if ns else None, ns, self._vec(out, self.q_hidden, "out"),
                 self._vec(lse, self.Hq, "lse") if lse is not None else None, self._scratch.data_ptr(),
                 rope_h.data_ptr() if fast else None, torch.cuda.current_stream().cuda_stream)
         if len_dev is None:
             vlut = self.vlut.data_ptr() if mha else None
-            _lib.check(self.lib.kvq_attend_gqa(*head, vlut, *vpart, *tail), "kvq_attend_gqa")
+            _lib.check(getattr(self.lib, "kvq_attend_gqa" + sfx)(*head, vlut, *vpart, *tail), "kvq_attend_gqa" + sfx)
         else:
-            _lib.check(self.lib.kvq_attend_gqa_dyn(*head, *vpart, self._vec(len_dev, 1, "len_dev", torch.int64),
-                                                   int(len_add), *tail), "kvq_attend_gqa_dyn")
+            _lib.check(getattr(self.lib, "kvq_attend_gqa_dyn" + sfx)(
+                *head, *vpart, self._vec(len_dev, 1, "len_dev", torch.int64), int(len_add), *tail),
+                "kvq_attend_gqa_dyn" + sfx)
         return out
 
     # -- device-resident length (one captured CUDA graph serves a growing cache; SURVEY.md 8(f)-2) ----------------------
@@ -334,14 +348,15 @@ class LayerCache:
             *self._out_ptrs("v"), s), "kvq_append_kv_fused_dyn")
 
     @_on_cache_device
-    def attend_dyn(self, q, len_dev, len_add=0, rope_theta=10000.0, out=None, lse=None, L_cap=None):
+    def attend_dyn(self, q, len_dev, len_add=0, rope_theta=10000.0, out=None, lse=None, L_cap=None, rope=None):
         """attend() over `min(len_dev[0] + len_add, L_cap)` slots, the length read on the device; grids, scratch and
-        the rope table are sized for L_cap (default: the whole allocation)."""
+        the rope table are sized for L_cap (default: the whole allocation).  rope: as attend()."""
         if self.group > 1:
             self._gqa_check()
         elif not self.use_native_v:
             raise NotImplementedError("device-resident length needs the native V form")
-        return self._attend(q, len_dev, len_add, rope_theta, out, lse, self.Lmax if L_cap is None else int(L_cap))
+        return self._attend(q, len_dev, len_add, _resolve_rope(rope, rope_theta), out, lse,
+                            self.Lmax if L_cap is None else int(L_cap))
 
     def _kv_out(self, t, n, name):
         """Caller-supplied fp16 [H, n, 128] output, possibly a view into a larger [H, S, 128] buffer: tokens and
@@ -361,7 +376,7 @@ class LayerCache:
         return t.stride(0)
 
     @_on_cache_device
-    def dequantize(self, start=0, stop=None, rope_theta=None, out_k=None, out_v=None):
+    def dequantize(self, start=0, stop=None, rope_theta=None, out_k=None, out_v=None, rope=None):
         """Slots [start, stop) of the cache as fp16 K and V, each [H, stop-start, 128] (one device pass, kvq_dequant_kv).
 
         K is the dequantised value (dequantisation table plus outlier residual); with rope_theta=None it is pre-RoPE,
@@ -370,7 +385,8 @@ class LayerCache:
         v_cent[code]*sf_t + off_t plus its outlier residual.  out_k / out_v may be views into larger [H, S, 128]
         buffers (stride (S*128, 128, 1)), each with its own S; an output not given is allocated.  An empty range
         returns empty outputs.  With both outputs given, and a rope table that already covers the range, the call
-        allocates nothing and can be captured in a CUDA graph."""
+        allocates nothing and can be captured in a CUDA graph.  rope (optional RotarySpec): rotate K with the spec's
+        table (scaled RoPE) in place of rope_theta's."""
         def call(start, stop, ok, ov, stride, rope, npos, pos_offset):
             _lib.check(self.lib.kvq_dequant_kv(
                 self.bits, self.H, self.Lmax, start, stop,
@@ -378,7 +394,8 @@ class LayerCache:
                 self.vcache.data_ptr(), self.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._out_ptrs("v"),
                 self.n_out, rope.data_ptr() if rope is not None else None, npos, pos_offset,
                 ok, ov, stride, torch.cuda.current_stream().cuda_stream), "kvq_dequant_kv")
-        return self._dequantize(start, stop, self.len, self.pos_base, rope_theta, out_k, out_v, call)
+        return self._dequantize(start, stop, self.len, self.pos_base, _resolve_rope(rope, rope_theta), out_k, out_v,
+                                call)
 
     def _dequantize(self, start, stop, n_cached, pos_base, rope_theta, out_k, out_v, call):
         """The body of dequantize for a cache of this one's shape holding n_cached tokens (this cache, or a slot of a
@@ -442,7 +459,7 @@ class LayerCache:
         return rope
 
     @_on_cache_device
-    def attend_chunk(self, q, k, v, rope_theta=10000.0):
+    def attend_chunk(self, q, k, v, rope_theta=10000.0, rope=None):
         """Causal attention of a T-token chunk placed right after the cached tokens (a follow-up prompt).
 
         q: f32 [T, q_heads, 128], token i already rotated at position P0 + i, P0 = n_sink + pos_base + len.
@@ -456,10 +473,12 @@ class LayerCache:
         position, 2*H*(n_sink + len + T)*128 fp16 values (2 GiB for 32 heads at 128K tokens), and hands them to
         torch.nn.functional.scaled_dot_product_attention.  attend_chunk_fused computes the same attention without
         materialising the cache.  A grouped-query cache hands the same H-head buffers to SDPA with enable_gqa=True
-        (nothing is repeated in memory)."""
+        (nothing is repeated in memory).  rope (optional RotarySpec): the cached and the chunk's keys are rotated with
+        the spec's table in place of rope_theta's; q must be rotated with the same spec."""
         if self.group > 1:
             self._gqa_check()
         self._chunk_check(q, k, v)
+        rope_theta = _resolve_rope(rope, rope_theta)
         sinks = (self.sink_k, self.sink_v) if self.sink_k is not None else None
         return self._attend_chunk_sdpa(q, k, v, rope_theta, self.len, self.pos_base, sinks,
                                        lambda ok, ov: self.dequantize(0, self.len, rope_theta, out_k=ok, out_v=ov))
@@ -488,7 +507,7 @@ class LayerCache:
         return out[0].transpose(0, 1).float().contiguous()
 
     @_on_cache_device
-    def attend_chunk_fused(self, q, k, v, rope_theta=10000.0):
+    def attend_chunk_fused(self, q, k, v, rope_theta=10000.0, rope=None):
         """attend_chunk() read straight from the quantised cache (kvq_attend_chunk): same arguments, checks, result
         (f32 [T, H, 128]) and semantics, and the cache is likewise left untouched.
 
@@ -496,12 +515,14 @@ class LayerCache:
         values dequantize() writes -- and attends the chunk over it, FlashAttention-2 style.  Extra device memory per
         call is the chunk's fp16 rotated K and V (2*H*T*128*2 bytes) plus kvq_attend_chunk_scratch_bytes(H, T, len),
         whatever `len` is: at 1M cached tokens the materialising attend_chunk would need 2*H*1M*128*2 bytes more.
-        A grouped-query cache calls kvq_attend_chunk_gqa (query head h reads KV head h // group)."""
+        A grouped-query cache calls kvq_attend_chunk_gqa (query head h reads KV head h // group).  rope: as
+        attend_chunk()."""
         if self.group > 1:
             self._gqa_check()
         if not self.use_native_v:
             raise NotImplementedError("attend_chunk_fused reads the native V form (use_native_v=True)")
         T = self._chunk_check(q, k, v)
+        rope_theta = _resolve_rope(rope, rope_theta)
         L = self.len
         ns = self.n_sink if self.sink_k is not None else 0
         pos_offset = self.n_sink + self.pos_base
@@ -619,14 +640,16 @@ class _BatchCommon:
             int(delta), self.B, torch.cuda.current_stream().cuda_stream), "kvq_dec_counter_add_batch")
 
     @_on_cache_device
-    def attend(self, q, out=None, lse=None, L_cap=None, len_add=0, rope_theta=10000.0):
+    def attend(self, q, out=None, lse=None, L_cap=None, len_add=0, rope_theta=10000.0, rope=None):
         """Decode attention of every sequence (kvq_attend_batch / kvq_attend_paged): q f32 [B, q_heads, 128], row b
         rotated at its own position; sequence b attends over its sinks and min(lens[b] + len_add, L_cap) slots (L_cap
         default: the per-sequence cap; grids, scratch and the rope table are sized for it).  Returns f32 [B, q_heads,
         128]; lse (optional f32 [B, q_heads]) receives the log-sum-exp.  An idle slot (no slot, no sink) gives 0 and
         -inf.  There is no active mask: with len_add > 0 a sequence that did not append this step attends one slot
-        past its length, so its output is meaningless and must be ignored."""
+        past its length, so its output is meaningless and must be ignored.  rope (optional RotarySpec): the keys'
+        rotary frequencies in place of rope_theta (kvq_attend_batch_freq / kvq_attend_paged_freq)."""
         c = self._tmpl
+        rope_theta = _resolve_rope(rope, rope_theta)
         if c.precision == "fp16":
             raise NotImplementedError("the batched attend uses the exact fp32 K tables (precision='fp32')")
         L_cap = self.Lmax if L_cap is None else int(L_cap)
@@ -644,14 +667,15 @@ class _BatchCommon:
         rope, _, npos = qc.rope_tables(self.device, rope_theta, L_cap + pos_offset + 1)
         out = self._out if out is None else out
         ns = self.n_sink if self.sink_k is not None else 0
+        sfx, rargs = _rope_call(self.device, rope_theta)
         args = (self.bits, self.B, self._rows(q, self.q_hidden, "q"), self.kcache.data_ptr(), c.klut_deq.data_ptr(),
                 *self._ptrs("k"), self.vcache.data_ptr(), c.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._ptrs("v"),
                 self.n_out, self.Hq, self.H, self._extent, L_cap, self.lens.data_ptr(), int(len_add), rope.data_ptr(),
-                npos, float(rope_theta), pos_offset, self.sink_k.data_ptr() if ns else None,
+                npos, *rargs, pos_offset, self.sink_k.data_ptr() if ns else None,
                 self.sink_v.data_ptr() if ns else None, ns, self._rows(out, self.q_hidden, "out"),
                 self._rows(lse, self.Hq, "lse") if lse is not None else None, self._scratch.data_ptr(), None,
                 torch.cuda.current_stream().cuda_stream) + self._page_args()
-        _lib.check(getattr(self.lib, self._attend_fn)(*args), self._attend_fn)
+        _lib.check(getattr(self.lib, self._attend_fn + sfx)(*args), self._attend_fn + sfx)
         return out
 
 
@@ -1094,11 +1118,13 @@ class PagedLayerCache(_BatchCommon):
                 ok, ov, stride, torch.cuda.current_stream().cuda_stream, *self._seq_args(b)), "kvq_dequant_kv_paged")
         return c._dequantize(start, stop, n_cached, 0, rope_theta, out_k, out_v, call)
 
-    def dequantize(self, b, start=0, stop=None, rope_theta=None, out_k=None, out_v=None):
+    def dequantize(self, b, start=0, stop=None, rope_theta=None, out_k=None, out_v=None, rope=None):
         """LayerCache.dequantize for slot b (kvq_dequant_kv_paged): slots [start, stop) of its lens_host[b] tokens as
-        fp16 K and V [H, stop - start, 128], the same values, with the same options, outputs and checks."""
+        fp16 K and V [H, stop - start, 128], the same values, with the same options (rope= included), outputs and
+        checks."""
         b = self.pages._slot(b)
-        return self._dequantize_at(b, start, stop, self.pages.lens_host[b], rope_theta, out_k, out_v)
+        return self._dequantize_at(b, start, stop, self.pages.lens_host[b], _resolve_rope(rope, rope_theta), out_k,
+                                   out_v)
 
     @_on_cache_device
     def _attend_chunk_at(self, b, L, q, k, v, rope_theta):
@@ -1110,12 +1136,12 @@ class PagedLayerCache(_BatchCommon):
         return c._attend_chunk_sdpa(q, k, v, rope_theta, L, 0, sinks,
                                     lambda ok, ov: self._dequantize_at(b, 0, L, L, rope_theta, ok, ov))
 
-    def attend_chunk(self, b, q, k, v, rope_theta=10000.0):
+    def attend_chunk(self, b, q, k, v, rope_theta=10000.0, rope=None):
         """LayerCache.attend_chunk for slot b: causal attention of a T-token chunk placed after the slot's lens_host[b]
-        tokens over its sinks, those tokens (dequantised in place, kvq_dequant_kv_paged) and the chunk; same arguments,
-        grouped-query rule and result, bit for bit.  The cache is not modified."""
+        tokens over its sinks, those tokens (dequantised in place, kvq_dequant_kv_paged) and the chunk; same arguments
+        (rope= included), grouped-query rule and result, bit for bit.  The cache is not modified."""
         b = self.pages._slot(b)
-        return self._attend_chunk_at(b, self.pages.lens_host[b], q, k, v, rope_theta)
+        return self._attend_chunk_at(b, self.pages.lens_host[b], q, k, v, _resolve_rope(rope, rope_theta))
 
     def slot(self, b):
         """Slot b as the single-sequence cache DecoderStage.prefill(caches=...) drives (PagedSlot)."""
@@ -1124,7 +1150,7 @@ class PagedLayerCache(_BatchCommon):
 
 class PagedSlot:
     """Slot b of a PagedLayerCache seen as one sequence's cache: what DecoderStage.prefill reads and calls -- len,
-    Lmax (the per-sequence cap), n_sink, pos_base (0), attend_chunk(q, k, v, rope_theta) and append_chunk(k, v).
+    Lmax (the per-sequence cap), n_sink, pos_base (0), attend_chunk(q, k, v, rope_theta, rope) and append_chunk(k, v).
 
     The layers of a batch share one PageTable and so one host length per slot, while a prompt goes through them one
     layer after the other.  So a handle keeps its own `len`, starting at the slot's lens_host[b]: attend_chunk attends
@@ -1137,8 +1163,8 @@ class PagedSlot:
         self.len = cache.pages.lens_host[self.b]
         self.Lmax, self.n_sink = cache.Lmax, cache.n_sink
 
-    def attend_chunk(self, q, k, v, rope_theta=10000.0):
-        return self.cache._attend_chunk_at(self.b, self.len, q, k, v, rope_theta)
+    def attend_chunk(self, q, k, v, rope_theta=10000.0, rope=None):
+        return self.cache._attend_chunk_at(self.b, self.len, q, k, v, _resolve_rope(rope, rope_theta))
 
     def append_chunk(self, k, v):
         self.len = self.cache._append_chunk_at(self.b, self.len, k, v)

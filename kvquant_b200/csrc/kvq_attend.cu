@@ -193,6 +193,8 @@ static int attend_validate(const AttendCall& c) {
   if (num_sms_cached() > kMaxPart) return KVQ_E_UNSUPPORTED;
   if (misaligned) return KVQ_E_ALIGN;
   if (bad_bits) return KVQ_E_BITS;
+  if (c.freq && !c.rope_freq) return KVQ_E_NULL;
+  if (c.freq && !(c.attn_factor > 0.f && c.attn_factor < INFINITY)) return KVQ_E_SHAPE;
   return 0;
 }
 
@@ -281,34 +283,49 @@ int kvq_attend_dyn(int bits, const float* q, const int32_t* kcache, const float*
   return rc ? rc : attend(c);
 }
 
-int kvq_attend_gqa(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-                   const int32_t* k_outlier_idx, const int32_t* vcache, const float* vlut_tok, const float* v_cent,
-                   const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv,
-                   int64_t Lmax, int64_t L, const float* rope_cos_sin, int64_t rope_npos, float theta, int pos_offset,
-                   const void* sink_k, const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
-                   const void* rope_half, void* stream) {
+}  // extern "C"
+
+// The rotary side of a call: theta (the kvq_attend* entry points) or a frequency vector and attention factor (their
+// *_freq siblings), stored into the AttendCall by the shared bodies below.
+struct RopeArg {
+  float theta;
+  const float* freq;
+  float attn;
+  bool scaled;
+  void set(AttendCall& c) const { c.theta = theta; c.freq = scaled; c.rope_freq = freq; c.attn_factor = attn; }
+};
+static RopeArg theta_arg(float theta) { return RopeArg{theta, nullptr, 1.f, false}; }
+static RopeArg freq_arg(const float* freq, float attn) { return RopeArg{0.f, freq, attn, true}; }
+
+static int attend_gqa(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
+                      const int32_t* k_outlier_idx, const int32_t* vcache, const float* vlut_tok, const float* v_cent,
+                      const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq,
+                      int Hkv, int64_t Lmax, int64_t L, const float* rope_cos_sin, int64_t rope_npos, RopeArg ra,
+                      int pos_offset, const void* sink_k, const void* sink_v, int n_sink, float* out, float* out_lse,
+                      void* scratch, const void* rope_half, void* stream) {
   AttendCall c{};
   c.bits = bits; c.q = q; c.kcache = kcache; c.klut = klut; c.k_outliers = k_outliers; c.k_outlier_idx = k_outlier_idx;
   c.vcache = vcache; c.vlut_tok = vlut_tok; c.v_cent = v_cent; c.v_aff = v_aff; c.v_outliers = v_outliers; c.v_outlier_idx = v_outlier_idx;
   c.n_out = n_out; c.Hq = Hq; c.Hkv = Hkv; c.Lmax = Lmax; c.L = L;
-  c.rope = rope_cos_sin; c.rope_half = rope_half; c.rope_npos = rope_npos; c.theta = theta; c.pos_offset = pos_offset;
+  c.rope = rope_cos_sin; c.rope_half = rope_half; c.rope_npos = rope_npos; ra.set(c); c.pos_offset = pos_offset;
   c.sink_k = sink_k; c.sink_v = sink_v; c.n_sink = n_sink; c.out = out; c.lse = out_lse; c.scratch = scratch;
   c.stream = static_cast<cudaStream_t>(stream);
   const int rc = check_gqa_call(c);
   return rc ? rc : attend(c);
 }
 
-int kvq_attend_gqa_dyn(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-                       const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
-                       const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax,
-                       int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
-                       int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
-                       float* out, float* out_lse, void* scratch, const void* rope_half, void* stream) {
+static int attend_gqa_dyn(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
+                          const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
+                          const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv,
+                          int64_t Lmax, int64_t L_cap, const int64_t* len_dev, int64_t len_add,
+                          const float* rope_cos_sin, int64_t rope_npos, RopeArg ra, int pos_offset, const void* sink_k,
+                          const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
+                          const void* rope_half, void* stream) {
   AttendCall c{};
   c.bits = bits; c.q = q; c.kcache = kcache; c.klut = klut; c.k_outliers = k_outliers; c.k_outlier_idx = k_outlier_idx;
   c.vcache = vcache; c.v_cent = v_cent; c.v_aff = v_aff; c.v_outliers = v_outliers; c.v_outlier_idx = v_outlier_idx;
   c.n_out = n_out; c.Hq = Hq; c.Hkv = Hkv; c.Lmax = Lmax; c.L = L_cap; c.len_dev = len_dev; c.len_add = len_add;
-  c.rope = rope_cos_sin; c.rope_half = rope_half; c.rope_npos = rope_npos; c.theta = theta; c.pos_offset = pos_offset;
+  c.rope = rope_cos_sin; c.rope_half = rope_half; c.rope_npos = rope_npos; ra.set(c); c.pos_offset = pos_offset;
   c.sink_k = sink_k; c.sink_v = sink_v; c.n_sink = n_sink; c.out = out; c.lse = out_lse; c.scratch = scratch;
   c.stream = static_cast<cudaStream_t>(stream);
   int rc = check_gqa_call(c);
@@ -318,18 +335,19 @@ int kvq_attend_gqa_dyn(int bits, const float* q, const int32_t* kcache, const fl
 
 // Batched decode attend: B sequences of one layer in one launch set, over a batch-strided cache of Lmax slots per
 // sequence
-int kvq_attend_batch(int bits, int B, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
-                     const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
-                     const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax,
-                     int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
-                     int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
-                     float* out, float* out_lse, void* scratch, const void* rope_half, void* stream) {
+static int attend_batch(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                        const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache,
+                        const float* v_cent, const float* v_aff, const float* v_outliers,
+                        const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax, int64_t L_cap,
+                        const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin, int64_t rope_npos,
+                        RopeArg ra, int pos_offset, const void* sink_k, const void* sink_v, int n_sink, float* out,
+                        float* out_lse, void* scratch, const void* rope_half, void* stream) {
   if (B < 1) return KVQ_E_SHAPE;
   AttendCall c{};
   c.bits = bits; c.q = q; c.kcache = kcache; c.klut = klut; c.k_outliers = k_outliers; c.k_outlier_idx = k_outlier_idx;
   c.vcache = vcache; c.v_cent = v_cent; c.v_aff = v_aff; c.v_outliers = v_outliers; c.v_outlier_idx = v_outlier_idx;
   c.n_out = n_out; c.Hq = Hq; c.Hkv = Hkv; c.Lmax = Lmax; c.L = L_cap; c.len_dev = len_dev; c.len_add = len_add;
-  c.rope = rope_cos_sin; c.rope_half = rope_half; c.rope_npos = rope_npos; c.theta = theta; c.pos_offset = pos_offset;
+  c.rope = rope_cos_sin; c.rope_half = rope_half; c.rope_npos = rope_npos; ra.set(c); c.pos_offset = pos_offset;
   c.sink_k = sink_k; c.sink_v = sink_v; c.n_sink = n_sink; c.out = out; c.lse = out_lse; c.scratch = scratch;
   c.stream = static_cast<cudaStream_t>(stream);
   c.B = B;
@@ -338,6 +356,101 @@ int kvq_attend_batch(int bits, int B, const float* q, const int32_t* kcache, con
 
 // Paged batch: the argument list of kvq_attend_batch with the pool size n_pool in place of Lmax, plus the page table;
 // the caches and row tensors are page pools and the per-sequence cap is max_pages * P
+static int attend_paged(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                        const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache,
+                        const float* v_cent, const float* v_aff, const float* v_outliers,
+                        const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int n_pool, int64_t L_cap,
+                        const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin, int64_t rope_npos,
+                        RopeArg ra, int pos_offset, const void* sink_k, const void* sink_v, int n_sink, float* out,
+                        float* out_lse, void* scratch, const void* rope_half, void* stream,
+                        const int32_t* page_table, int max_pages, const int32_t* npages, int P) {
+  if (B < 1) return KVQ_E_SHAPE;
+  const PageRef pg{page_table, npages, max_pages, P, n_pool};
+  AttendCall c{};
+  c.bits = bits; c.q = q; c.kcache = kcache; c.klut = klut; c.k_outliers = k_outliers; c.k_outlier_idx = k_outlier_idx;
+  c.vcache = vcache; c.v_cent = v_cent; c.v_aff = v_aff; c.v_outliers = v_outliers; c.v_outlier_idx = v_outlier_idx;
+  c.n_out = n_out; c.Hq = Hq; c.Hkv = Hkv; c.Lmax = (int64_t)max_pages * P; c.L = L_cap; c.len_dev = len_dev; c.len_add = len_add;
+  c.rope = rope_cos_sin; c.rope_half = rope_half; c.rope_npos = rope_npos; ra.set(c); c.pos_offset = pos_offset;
+  c.sink_k = sink_k; c.sink_v = sink_v; c.n_sink = n_sink; c.out = out; c.lse = out_lse; c.scratch = scratch;
+  c.stream = static_cast<cudaStream_t>(stream);
+  c.B = B; c.pg = &pg;
+  return attend(c);
+}
+
+extern "C" {
+
+#define KVQ_GQA_ARGS(ROPE)                                                                                               \
+  bits, q, kcache, klut, k_outliers, k_outlier_idx, vcache, vlut_tok, v_cent, v_aff, v_outliers, v_outlier_idx, n_out,   \
+      Hq, Hkv, Lmax, L, rope_cos_sin, rope_npos, ROPE, pos_offset, sink_k, sink_v, n_sink, out, out_lse, scratch,       \
+      rope_half, stream
+#define KVQ_DYN_ARGS(ROPE)                                                                                               \
+  bits, q, kcache, klut, k_outliers, k_outlier_idx, vcache, v_cent, v_aff, v_outliers, v_outlier_idx, n_out, Hq, Hkv,    \
+      Lmax, L_cap, len_dev, len_add, rope_cos_sin, rope_npos, ROPE, pos_offset, sink_k, sink_v, n_sink, out, out_lse,   \
+      scratch, rope_half, stream
+#define KVQ_BATCH_ARGS(EXTENT, ROPE)                                                                                     \
+  bits, B, q, kcache, klut, k_outliers, k_outlier_idx, vcache, v_cent, v_aff, v_outliers, v_outlier_idx, n_out, Hq, Hkv, \
+      EXTENT, L_cap, len_dev, len_add, rope_cos_sin, rope_npos, ROPE, pos_offset, sink_k, sink_v, n_sink, out, out_lse, \
+      scratch, rope_half, stream
+
+int kvq_attend_gqa(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
+                   const int32_t* k_outlier_idx, const int32_t* vcache, const float* vlut_tok, const float* v_cent,
+                   const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv,
+                   int64_t Lmax, int64_t L, const float* rope_cos_sin, int64_t rope_npos, float theta, int pos_offset,
+                   const void* sink_k, const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
+                   const void* rope_half, void* stream) {
+  return attend_gqa(KVQ_GQA_ARGS(theta_arg(theta)));
+}
+
+int kvq_attend_gqa_freq(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
+                        const int32_t* k_outlier_idx, const int32_t* vcache, const float* vlut_tok, const float* v_cent,
+                        const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq,
+                        int Hkv, int64_t Lmax, int64_t L, const float* rope_cos_sin, int64_t rope_npos,
+                        const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                        const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
+                        const void* rope_half, void* stream) {
+  return attend_gqa(KVQ_GQA_ARGS(freq_arg(rope_freq, attn_factor)));
+}
+
+int kvq_attend_gqa_dyn(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
+                       const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
+                       const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax,
+                       int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
+                       int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
+                       float* out, float* out_lse, void* scratch, const void* rope_half, void* stream) {
+  return attend_gqa_dyn(KVQ_DYN_ARGS(theta_arg(theta)));
+}
+
+int kvq_attend_gqa_dyn_freq(int bits, const float* q, const int32_t* kcache, const float* klut,
+                            const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache,
+                            const float* v_cent, const float* v_aff, const float* v_outliers,
+                            const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax, int64_t L_cap,
+                            const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin, int64_t rope_npos,
+                            const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                            const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
+                            const void* rope_half, void* stream) {
+  return attend_gqa_dyn(KVQ_DYN_ARGS(freq_arg(rope_freq, attn_factor)));
+}
+
+int kvq_attend_batch(int bits, int B, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
+                     const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
+                     const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax,
+                     int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
+                     int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
+                     float* out, float* out_lse, void* scratch, const void* rope_half, void* stream) {
+  return attend_batch(KVQ_BATCH_ARGS(Lmax, theta_arg(theta)));
+}
+
+int kvq_attend_batch_freq(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                          const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache,
+                          const float* v_cent, const float* v_aff, const float* v_outliers,
+                          const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax, int64_t L_cap,
+                          const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin, int64_t rope_npos,
+                          const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                          const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
+                          const void* rope_half, void* stream) {
+  return attend_batch(KVQ_BATCH_ARGS(Lmax, freq_arg(rope_freq, attn_factor)));
+}
+
 int kvq_attend_paged(int bits, int B, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
                      const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent, const float* v_aff,
                      const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int n_pool,
@@ -345,17 +458,19 @@ int kvq_attend_paged(int bits, int B, const float* q, const int32_t* kcache, con
                      int64_t rope_npos, float theta, int pos_offset, const void* sink_k, const void* sink_v, int n_sink,
                      float* out, float* out_lse, void* scratch, const void* rope_half, void* stream,
                      const int32_t* page_table, int max_pages, const int32_t* npages, int P) {
-  if (B < 1) return KVQ_E_SHAPE;
-  const PageRef pg{page_table, npages, max_pages, P, n_pool};
-  AttendCall c{};
-  c.bits = bits; c.q = q; c.kcache = kcache; c.klut = klut; c.k_outliers = k_outliers; c.k_outlier_idx = k_outlier_idx;
-  c.vcache = vcache; c.v_cent = v_cent; c.v_aff = v_aff; c.v_outliers = v_outliers; c.v_outlier_idx = v_outlier_idx;
-  c.n_out = n_out; c.Hq = Hq; c.Hkv = Hkv; c.Lmax = (int64_t)max_pages * P; c.L = L_cap; c.len_dev = len_dev; c.len_add = len_add;
-  c.rope = rope_cos_sin; c.rope_half = rope_half; c.rope_npos = rope_npos; c.theta = theta; c.pos_offset = pos_offset;
-  c.sink_k = sink_k; c.sink_v = sink_v; c.n_sink = n_sink; c.out = out; c.lse = out_lse; c.scratch = scratch;
-  c.stream = static_cast<cudaStream_t>(stream);
-  c.B = B; c.pg = &pg;
-  return attend(c);
+  return attend_paged(KVQ_BATCH_ARGS(n_pool, theta_arg(theta)), page_table, max_pages, npages, P);
+}
+
+int kvq_attend_paged_freq(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                          const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache,
+                          const float* v_cent, const float* v_aff, const float* v_outliers,
+                          const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int n_pool, int64_t L_cap,
+                          const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin, int64_t rope_npos,
+                          const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                          const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
+                          const void* rope_half, void* stream, const int32_t* page_table, int max_pages,
+                          const int32_t* npages, int P) {
+  return attend_paged(KVQ_BATCH_ARGS(n_pool, freq_arg(rope_freq, attn_factor)), page_table, max_pages, npages, P);
 }
 
 int kvq_attend_merge(const float* parts, int n_parts, int H, float* out, void* stream) {

@@ -39,6 +39,9 @@ struct AttendCall {
   const void* rope_half;             // half2 copy of it: selects the fp16-table K form; null = exact fp32
   int64_t rope_npos;
   float theta;
+  bool freq;                         // the *_freq entry points: the table was built from rope_freq and attn_factor
+  const float* rope_freq;            // f32 [64] (device): the outlier pass's rotary frequencies, theta unused
+  float attn_factor;
   int pos_offset;
   const void* sink_k;
   const void* sink_v;

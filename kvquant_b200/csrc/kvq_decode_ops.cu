@@ -84,6 +84,32 @@ __global__ void dec_rope_split_batch_kernel(const __half* __restrict__ qkv, cons
   }
 }
 
+// scaled rotary frequencies (kvq_dec_rope_split_freq): row b rotated at pos_add (+ pos_dev[b] when given) with
+// cos / sin times attn -- HF's attention_factor, applied to the query as to the keys (rope_table_freq_kernel)
+__global__ void dec_rope_split_freq_kernel(const __half* __restrict__ qkv, const float* __restrict__ inv_freq, float attn,
+                                           float pos_add, const int64_t* __restrict__ pos_dev, float* __restrict__ q,
+                                           float* __restrict__ k, float* __restrict__ v, int hidden, int kv_hidden) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= hidden) return;
+  const int64_t r = blockIdx.y;
+  qkv += r * (hidden + 2 * kv_hidden);
+  q += r * hidden; k += r * kv_hidden; v += r * kv_hidden;
+  const float pos = pos_dev != nullptr ? pos_add + (float)pos_dev[r] : pos_add;
+  const int c = i & (kHeadDim - 1), j = c & (kHalf - 1);
+  const float ang = inv_freq[j] * pos;
+  float sn, cs;
+  sincosf(ang, &sn, &cs);
+  cs *= attn;
+  sn *= attn;
+  const float a = __half2float(qkv[i]);
+  const float b = __half2float(qkv[i ^ kHalf]);
+  q[i] = a * cs + ((c < kHalf) ? -b : b) * sn;
+  if (i < kv_hidden) {
+    k[i] = __half2float(qkv[hidden + i]);
+    v[i] = __half2float(qkv[hidden + kv_hidden + i]);
+  }
+}
+
 // counter[b] += delta for every b with active[b] != 0 (active == null: every b)
 __global__ void dec_counter_add_batch_kernel(int64_t* c, const int32_t* __restrict__ active, int64_t d, int B) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -170,6 +196,18 @@ int kvq_dec_rope_split_batch(const void* qkv_f16, const float* inv_freq, const i
   const int hidden = Hq * kHeadDim;
   dec_rope_split_batch_kernel<<<dim3((hidden + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __half*>(qkv_f16), inv_freq, (float)pos_add, pos_dev, q, k, v, hidden, Hkv * kHeadDim);
+  KVQ_LAUNCH_CHECK();
+  return 0;
+}
+
+int kvq_dec_rope_split_freq(const void* qkv_f16, const float* inv_freq, float attn_factor, const int64_t* pos_dev,
+                            int64_t pos_add, float* q, float* k, float* v, int Hq, int Hkv, int B, void* stream) {
+  if (!qkv_f16 || !inv_freq || !q || !k || !v) return KVQ_E_NULL;
+  if (check_split_gqa(Hq, Hkv) || B < 1 || B > 65535) return KVQ_E_SHAPE;
+  if (!(attn_factor > 0.f && attn_factor < INFINITY)) return KVQ_E_SHAPE;
+  const int hidden = Hq * kHeadDim;
+  dec_rope_split_freq_kernel<<<dim3((hidden + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const __half*>(qkv_f16), inv_freq, attn_factor, (float)pos_add, pos_dev, q, k, v, hidden, Hkv * kHeadDim);
   KVQ_LAUNCH_CHECK();
   return 0;
 }

@@ -278,15 +278,20 @@ __global__ void __launch_bounds__(kOutThreads) k_outlier_kernel(
 // read from row page_of(b, t) * P + t % P, and the length is also capped at npages[b] * P.  Others ignore `pg`.
 constexpr int kOutPersThreads = 512;
 constexpr size_t kOutThetaBytes = kHalf * sizeof(float);   // dynamic shared memory past the q table: s_th
-template <bool GQA, bool BATCH, bool PAGED = false>
-__global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
+//
+// FREQ (k_outlier_pers_freq_kernel): scaled rotary frequencies (DESIGN.md section 4.13).  The computed factors use
+// f_j = rope_freq[j] in place of rope_row_theta(rope_theta, j), times attn, as rope_table_freq_kernel builds the table;
+// rope_freq == null gathers every factor from the table (the wrapper passes rope_theta = 1 or 0 for given or null).
+template <bool GQA, bool BATCH, bool PAGED, bool FREQ>
+__device__ __forceinline__ void k_outlier_pers_body(
     const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
     float* __restrict__ out, int64_t stride_h, int64_t stride_t, int64_t L, int H, int n_out,
     const float2* __restrict__ rope, int64_t rope_npos, int pos_offset, float scale,
     const int64_t* __restrict__ len_dev, int64_t len_add, const uint32_t* __restrict__ rope_h, float rope_theta, int grp,
-    const int64_t b_out, const int64_t b_rows, const PageRef pg) {
+    const int64_t b_out, const int64_t b_rows, const PageRef pg, const float* __restrict__ rope_freq, float attn) {
   extern __shared__ float2 s_qq[];                       // [H*128] = (q[c], q[c^64]), query heads
-  float* const s_th = reinterpret_cast<float*>(s_qq + H * kHeadDim);   // [64]: theta_j of rotary row j (rope_theta > 0)
+  float* const s_th = reinterpret_cast<float*>(s_qq + H * kHeadDim);   // [64]: theta_j of rotary row j (direct)
+  const bool direct = rope_theta > 0.f;
   if constexpr (BATCH) {
     const int b = blockIdx.y;
     q += (int64_t)b * H * kHeadDim;
@@ -305,7 +310,11 @@ __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
   const uint32_t total = (uint32_t)(L * n_out);          // host checks L * n_out < 2^31
   const int tid = threadIdx.x, lane = tid & 31;
   for (int i = tid; i < H * kHeadDim; i += kOutPersThreads) s_qq[i] = make_float2(q[i], q[i ^ kHalf]);
-  if (rope_theta > 0.f && tid < kHalf) s_th[tid] = rope_row_theta(rope_theta, tid);
+  if constexpr (FREQ) {
+    if (direct && tid < kHalf) s_th[tid] = rope_freq[tid];
+  } else {
+    if (direct && tid < kHalf) s_th[tid] = rope_row_theta(rope_theta, tid);
+  }
   __syncthreads();
   const uint32_t stride = gridDim.x * kOutPersThreads;
   // outlier rows are read once: evict them first, so that the score rows the atomics add into (just cleared) stay in L2
@@ -336,7 +345,7 @@ __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
       key = (int)(t * 64u) + h;                          // t < 2^25
       if (v != 0.f) {   // pads / non-outliers contribute exactly 0 in the reference too
         float2 cs;
-        if (rope_theta > 0.f) {
+        if (direct) {
           // the table builder's own expressions (same device functions, same arguments: bit-identical values) cost
           // less than a scattered 8-byte gather, which past L2-sized tables is a 32-byte DRAM sector.  Past
           // CUDART_TRIG_PLOSS_F, cosf / sinf leave their fast argument reduction for a local-memory one that stalls
@@ -344,8 +353,13 @@ __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
           // stay in L2.
           const int j = c & (kHalf - 1), pos = (int)t + pos_offset;
           const float th = s_th[j];
-          if (th * pos <= CUDART_TRIG_PLOSS_F) cs = rope_cos_sin(th, pos);
+          const bool fast = th * pos <= CUDART_TRIG_PLOSS_F;
+          if (fast) cs = rope_cos_sin(th, pos);
           else cs = ld_keep_f2(rope + (int64_t)j * rope_npos + pos, pol_keep);
+          if constexpr (FREQ) {   // the table's entries already carry attn (a product with 1 is exact)
+            const float m = fast ? attn : 1.f;
+            cs = make_float2(cs.x * m, cs.y * m);
+          }
         } else if (rope_h != nullptr) {   // fp16 mode: the half2 table the dense kernel streams (half the bytes per gather)
           uint32_t u;
           asm volatile("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(u)
@@ -396,6 +410,31 @@ __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
   }
 }
 
+template <bool GQA, bool BATCH, bool PAGED = false>
+__global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
+    const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
+    float* __restrict__ out, int64_t stride_h, int64_t stride_t, int64_t L, int H, int n_out,
+    const float2* __restrict__ rope, int64_t rope_npos, int pos_offset, float scale,
+    const int64_t* __restrict__ len_dev, int64_t len_add, const uint32_t* __restrict__ rope_h, float rope_theta, int grp,
+    const int64_t b_out, const int64_t b_rows, const PageRef pg) {
+  k_outlier_pers_body<GQA, BATCH, PAGED, false>(q, outliers, outlier_idx, out, stride_h, stride_t, L, H, n_out, rope,
+                                                rope_npos, pos_offset, scale, len_dev, len_add, rope_h, rope_theta, grp,
+                                                b_out, b_rows, pg, nullptr, 1.f);
+}
+
+template <bool GQA, bool BATCH, bool PAGED = false>
+__global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_freq_kernel(
+    const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
+    float* __restrict__ out, int64_t stride_h, int64_t stride_t, int64_t L, int H, int n_out,
+    const float2* __restrict__ rope, int64_t rope_npos, int pos_offset, float scale,
+    const int64_t* __restrict__ len_dev, int64_t len_add, const uint32_t* __restrict__ rope_h,
+    const float* __restrict__ rope_freq, float attn, int grp, const int64_t b_out, const int64_t b_rows, const PageRef pg) {
+  k_outlier_pers_body<GQA, BATCH, PAGED, true>(q, outliers, outlier_idx, out, stride_h, stride_t, L, H, n_out, rope,
+                                               rope_npos, pos_offset, scale, len_dev, len_add, rope_h,
+                                               rope_freq != nullptr ? 1.f : 0.f, grp,
+                                               b_out, b_rows, pg, rope_freq, attn);
+}
+
 static int k_out_impl_table() {   // KVQ_KOUT_IMPL=table selects the non-persistent gather form for A/B runs
   static int v = -1;
   if (v < 0) { const char* e = getenv("KVQ_KOUT_IMPL"); v = (e && e[0] == 't') ? 1 : 0; }
@@ -413,15 +452,18 @@ static bool k_out_direct(int64_t n_positions, bool half_table) {
   return n_positions > (thr >= 0 ? thr : (half_table ? 64 * 1024 : 0));
 }
 
-static int set_k_outlier_smem(size_t smem, bool gqa, bool batch, bool paged) {
-  static size_t smem_set_dev[6][64];   // per kernel and device: largest dynamic shared memory opted in so far (0 = 48 KiB)
+static int set_k_outlier_smem(size_t smem, bool gqa, bool batch, bool paged, bool freq = false) {
+  static size_t smem_set_dev[12][64];  // per kernel and device: largest dynamic shared memory opted in so far (0 = 48 KiB)
   int dev_idx = 0;
   cudaGetDevice(&dev_idx);
-  size_t& smem_set = smem_set_dev[gqa + 2 * (batch + paged)][dev_idx & 63];
+  size_t& smem_set = smem_set_dev[gqa + 2 * (batch + paged) + 6 * freq][dev_idx & 63];
   if (smem_set == 0) smem_set = 48 * 1024;
   if (smem > smem_set) {
     const cudaError_t e = with_flavour(gqa, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
-      return cudaFuncSetAttribute(k_outlier_pers_kernel<GQA(), BATCH(), PAGED()>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      return freq ? cudaFuncSetAttribute(k_outlier_pers_freq_kernel<GQA(), BATCH(), PAGED()>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                  : cudaFuncSetAttribute(k_outlier_pers_kernel<GQA(), BATCH(), PAGED()>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     });
     if (e != cudaSuccess) return (int)e;
     smem_set = smem;
@@ -452,14 +494,20 @@ static int launch_k_outliers(const KParams& p, cudaStream_t st) {
     KVQ_LAUNCH_CHECK();
     return 0;
   }
-  const int rc = set_k_outlier_smem(smem + kOutThetaBytes, gqa, false, false);
+  const int rc = set_k_outlier_smem(smem + kOutThetaBytes, gqa, false, false, p.freq);
   if (rc != 0) return rc;
   const unsigned grid = k_outlier_grid(total, smem, 1);
-  const float direct_theta = k_out_direct(p.L + p.pos_offset, p.rope_h != nullptr) ? p.theta : 0.f;
+  const bool direct = k_out_direct(p.L + p.pos_offset, p.rope_h != nullptr);
+  const float direct_theta = direct ? p.theta : 0.f;
   with_flavour(gqa, false, false, [&](auto GQA, auto BATCH, auto PAGED) {
-    k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, st>>>(
-        p.q, p.outliers, p.outlier_idx, p.out, p.out_stride, 1, p.L, p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset, 1.f,
-        p.len_dev, p.len_add, p.rope_h, direct_theta, gqa ? p.grp : 1, 0, 0, PageRef{});
+    if (p.freq)
+      k_outlier_pers_freq_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, st>>>(
+          p.q, p.outliers, p.outlier_idx, p.out, p.out_stride, 1, p.L, p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset,
+          1.f, p.len_dev, p.len_add, p.rope_h, direct ? p.rope_freq : nullptr, p.attn, gqa ? p.grp : 1, 0, 0, PageRef{});
+    else
+      k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, st>>>(
+          p.q, p.outliers, p.outlier_idx, p.out, p.out_stride, 1, p.L, p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset, 1.f,
+          p.len_dev, p.len_add, p.rope_h, direct_theta, gqa ? p.grp : 1, 0, 0, PageRef{});
   });
   KVQ_LAUNCH_CHECK();
   return 0;
@@ -471,6 +519,24 @@ __global__ void rope_table_kernel(float2* __restrict__ out, float rope_theta, in
   const float theta = rope_row_theta(rope_theta, j);
   for (int64_t pos64 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos64 < n_pos; pos64 += (int64_t)gridDim.x * blockDim.x)
     out[(int64_t)j * n_pos + pos64] = rope_cos_sin(theta, (int)pos64);
+}
+
+// scaled rope table: (cosf(f_j p) * attn, sinf(f_j p) * attn), f_j = freq[j] -- the factors k_outlier_pers_freq_kernel
+// computes.  HALF: the same values rounded once to fp16 (half2 entries).
+template <bool HALF>
+__global__ void rope_table_freq_kernel(void* __restrict__ out, const float* __restrict__ freq, float attn, int64_t n_pos) {
+  const int j = blockIdx.y;
+  const float f = freq[j];
+  for (int64_t pos64 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos64 < n_pos; pos64 += (int64_t)gridDim.x * blockDim.x) {
+    const float2 cs = rope_cos_sin(f, (int)pos64);
+    const float2 e = make_float2(cs.x * attn, cs.y * attn);
+    if constexpr (HALF) {
+      const __half2 h = __floats2half2_rn(e.x, e.y);
+      static_cast<uint32_t*>(out)[(int64_t)j * n_pos + pos64] = *reinterpret_cast<const uint32_t*>(&h);
+    } else {
+      static_cast<float2*>(out)[(int64_t)j * n_pos + pos64] = e;
+    }
+  }
 }
 
 template <int BITS>
@@ -523,6 +589,7 @@ int k_scores_fused(const AttendCall& c, const AttendScratch& s) {
     p.H = c.Hq; p.n_out = c.n_out; p.pos_offset = c.pos_offset; p.theta = c.theta;
     p.outliers = c.k_outliers; p.outlier_idx = c.k_outlier_idx;
     p.rope_h = static_cast<const uint32_t*>(c.rope_half); p.grp = c.grp();
+    p.freq = c.freq; p.rope_freq = c.rope_freq; p.attn = c.attn_factor;
     cudaError_t e = cudaMemset2DAsync(s.scores, sizeof(float) * (size_t)s.stride, 0, sizeof(float) * (size_t)c.L, (size_t)c.Hq, c.stream);
     if (e != cudaSuccess) return (int)e;
     const int rc = launch_k_outliers(p, c.stream);
@@ -557,16 +624,23 @@ int k_scores_batch(const AttendCall& c, const AttendScratch& s) {
     k_batch_zero_kernel<<<dim3((unsigned)std::min<int64_t>((c.L + 2047) / 2048, 64), H, B), 256, 0, c.stream>>>(
         s.scores, s.stride, s.bstride, c.len_dev, c.len_add, c.L);
     KVQ_LAUNCH_CHECK();
-    const int rc = set_k_outlier_smem(smem + kOutThetaBytes, grp > 1, true, c.pg != nullptr);
+    const int rc = set_k_outlier_smem(smem + kOutThetaBytes, grp > 1, true, c.pg != nullptr, c.freq);
     if (rc != 0) return rc;
     const dim3 grid(k_outlier_grid(c.L * c.n_out, smem, B), (unsigned)B);
-    const float direct_theta = k_out_direct(c.L + c.pos_offset, false) ? c.theta : 0.f;
+    const bool direct = k_out_direct(c.L + c.pos_offset, false);
+    const float direct_theta = direct ? c.theta : 0.f;
     const int64_t b_rows = c.pg != nullptr ? 0 : c.Lmax * c.n_out;   // a pool has no per-sequence row block
+    const float2* rope = reinterpret_cast<const float2*>(c.rope);
+    const PageRef pg = c.pg != nullptr ? *c.pg : PageRef{};
     with_flavour(grp > 1, true, c.pg != nullptr, [&](auto GQA, auto BATCH, auto PAGED) {
-      k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
-          c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, reinterpret_cast<const float2*>(c.rope),
-          c.rope_npos, c.pos_offset, 1.f, c.len_dev, c.len_add, nullptr, direct_theta, grp, s.bstride, b_rows,
-          c.pg != nullptr ? *c.pg : PageRef{});
+      if (c.freq)
+        k_outlier_pers_freq_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
+            c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, rope, c.rope_npos, c.pos_offset,
+            1.f, c.len_dev, c.len_add, nullptr, direct ? c.rope_freq : nullptr, c.attn_factor, grp, s.bstride, b_rows, pg);
+      else
+        k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
+            c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, rope, c.rope_npos, c.pos_offset,
+            1.f, c.len_dev, c.len_add, nullptr, direct_theta, grp, s.bstride, b_rows, pg);
     });
     KVQ_LAUNCH_CHECK();
     accumulate = 1;
@@ -587,6 +661,25 @@ int kvq_rope_table_build(float* rope_cos_sin, float theta, int64_t n_pos, void* 
   rope_table_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(reinterpret_cast<float2*>(rope_cos_sin), theta, n_pos);
   KVQ_LAUNCH_CHECK();
   return 0;
+}
+
+// scaled tables: every argument is checked before anything is launched, the frequency vector is read on the device
+static int rope_table_freq_build(void* out, const float* freq, float attn_factor, int64_t n_pos, void* stream, bool half) {
+  if (!out || !freq) return KVQ_E_NULL;
+  if (n_pos <= 0 || n_pos > (int64_t)1 << 30 || !(attn_factor > 0.f && attn_factor < INFINITY)) return KVQ_E_SHAPE;
+  const dim3 grid((unsigned)((n_pos + 255) / 256 > 4096 ? 4096 : (n_pos + 255) / 256), kHalf);
+  if (half) rope_table_freq_kernel<true><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(out, freq, attn_factor, n_pos);
+  else rope_table_freq_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(out, freq, attn_factor, n_pos);
+  KVQ_LAUNCH_CHECK();
+  return 0;
+}
+
+int kvq_rope_table_build_freq(float* rope_cos_sin, const float* freq, float attn_factor, int64_t n_pos, void* stream) {
+  return rope_table_freq_build(rope_cos_sin, freq, attn_factor, n_pos, stream, false);
+}
+
+int kvq_rope_table_build_freq_half(void* rope_half, const float* freq, float attn_factor, int64_t n_pos, void* stream) {
+  return rope_table_freq_build(rope_half, freq, attn_factor, n_pos, stream, true);
 }
 
 int kvq_k_matvec(int bits, const float* q, const int32_t* cache, float* mul, const float* lut, int B, int H,

@@ -21,6 +21,9 @@ struct KParams {
   const uint32_t* rope_h;    // optional half2 copy of the rope table (fp16 mode of the fused attend: the outlier scatter
                              // gathers 4-byte entries from the table the dense kernel streams anyway)
   int grp;                   // query heads per KV head (H counts query heads; the fused attend's outlier pass only)
+  bool freq;                 // scaled rotary frequencies: the outlier pass computes cos / sin of rope_freq[j] * pos,
+  const float* rope_freq;    // times attn, instead of using theta (the fused attend's outlier pass only)
+  float attn;
 };
 
 // compile-time loop (immediate LDS offsets and PRMT selectors need constant expressions)

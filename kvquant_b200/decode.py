@@ -27,6 +27,7 @@ from dataclasses import dataclass
 import torch
 
 from .cache import BatchedLayerCache, LayerCache, PagedLayerCache, PageTable, HEAD_DIM
+from .rope import RotarySpec
 
 
 @dataclass
@@ -45,6 +46,7 @@ class DecodeConfig:
     sparse_v: bool = True      # False: outlier rows for K only (BASELINE configs[4]: capped K outliers)
     max_len: int = 4096        # quantised slots allocated per layer
     n_kv_heads: int = None     # grouped-query attention: KV heads (None: n_heads); query head h reads KV head h // g
+    rope_scaling: dict = None  # HF rope_scaling dict ("linear", "llama3", "yarn"); None: plain rope_theta frequencies
 
     @property
     def kv_heads(self):
@@ -53,6 +55,12 @@ class DecodeConfig:
     @property
     def kv_hidden(self):
         return self.kv_heads * HEAD_DIM
+
+    @property
+    def rotary(self):
+        """The scaled RotarySpec of rope_theta + rope_scaling, or None for the plain-theta frequencies."""
+        spec = RotarySpec(self.rope_theta, self.rope_scaling)
+        return spec if spec.scaled else None
 
     @staticmethod
     def llama7b(**kw):
@@ -69,6 +77,15 @@ class DecodeConfig:
                    n_kv_heads=8)
         cfg.update(kw)
         return DecodeConfig(**cfg)
+
+    @staticmethod
+    def llama31_8b(**kw):
+        """LLaMA-3.1-8B: the llama3_8b shapes with LLaMA-3.1's rotary scaling (rope_type "llama3", factor 8, original
+        context 8192)."""
+        cfg = dict(rope_scaling={"rope_type": "llama3", "factor": 8.0, "low_freq_factor": 1.0, "high_freq_factor": 4.0,
+                                 "original_max_position_embeddings": 8192})
+        cfg.update(kw)
+        return DecodeConfig.llama3_8b(**cfg)
 
 
 def partition_layers(n_layers: int, world: int, rank: int):
@@ -117,6 +134,9 @@ class DecoderStage:
         Grouped-query models (cfg.n_kv_heads) run unsharded only."""
         if sp is not None and cfg.kv_heads != cfg.n_heads:
             raise NotImplementedError("sequence-sharded attention of a grouped-query model")
+        self.rotary = cfg.rotary   # scaled RotarySpec, or None: rope_theta's frequencies
+        if sp is not None and self.rotary is not None:
+            raise NotImplementedError("sequence-sharded attention with scaled rotary frequencies")
         self.cfg, self.lo, self.hi = cfg, lo, hi
         self.device = torch.device(device)
         self.sp = sp
@@ -133,7 +153,10 @@ class DecoderStage:
             self.norm = torch.ones(cfg.hidden, dtype=torch.float16, device=self.device)
             self.lm_head = (torch.randn((cfg.vocab, cfg.hidden), generator=gen, device=self.device) * 0.02).half()
         half = HEAD_DIM // 2
-        self.inv_freq = 1.0 / (cfg.rope_theta ** (torch.arange(0, HEAD_DIM, 2, device=self.device).float() / HEAD_DIM))
+        if self.rotary is None:
+            self.inv_freq = 1.0 / (cfg.rope_theta ** (torch.arange(0, HEAD_DIM, 2, device=self.device).float() / HEAD_DIM))
+        else:   # HF's inv_freq, the vector the caches' tables are built from
+            self.inv_freq = self.rotary.inv_freq.to(self.device)
         self._half = half
 
     # -- pieces -------------------------------------------------------------------------------------------------
@@ -150,6 +173,8 @@ class DecoderStage:
         ang = self.inv_freq * float(pos)
         cos = torch.cat((ang.cos(), ang.cos()))
         sin = torch.cat((ang.sin(), ang.sin()))
+        if self.rotary is not None:     # HF multiplies cos and sin by the attention factor (YaRN)
+            cos, sin = cos * self.rotary.attention_factor, sin * self.rotary.attention_factor
         rot = torch.cat((-q[:, self._half:], q[:, :self._half]), dim=-1)
         return q * cos + rot * sin
 
@@ -200,7 +225,13 @@ class DecoderStage:
             c = ly.cache
             dyn = self.dyn          # device-resident length / position (one graph for a growing cache) or None
             self._gemv(ly.wqkv, x, 3, b["qkv"], norm_w=ly.n1)
-            if dyn is None:
+            if self.rotary is not None:   # (unsharded): position *pos_dev, or the host position
+                pos = (dyn["pos"].data_ptr(), 0) if dyn is not None else (None, c.n_sink + c.pos_base + c.len)
+                _lib.check(lib.kvq_dec_rope_split_freq(b["qkv"].data_ptr(), self.inv_freq.data_ptr(),
+                                                       self.rotary.attention_factor, *pos, b["q"].data_ptr(),
+                                                       b["k"].data_ptr(), b["v"].data_ptr(), H, cfg.kv_heads, 1, st),
+                           "kvq_dec_rope_split_freq")
+            elif dyn is None:
                 # absolute position of the new token
                 pos = self.global_pos if self.sp is not None else c.n_sink + c.pos_base + c.len
                 qkv = (b["qkv"].data_ptr(), self.inv_freq.data_ptr(), float(pos),
@@ -216,10 +247,10 @@ class DecoderStage:
             if self.sp is None:
                 if dyn is None:
                     c.append(b["k"], b["v"])             # pre-RoPE K, per-token V: quantise + outlier split
-                    o = c.attend(qh, rope_theta=cfg.rope_theta)   # f32 [H,128]
+                    o = c.attend(qh, rope_theta=cfg.rope_theta, rope=self.rotary)   # f32 [H,128]
                 else:
                     c.append_dyn(b["k"], b["v"], dyn["len"])
-                    o = c.attend_dyn(qh, dyn["len"], 1, rope_theta=cfg.rope_theta)
+                    o = c.attend_dyn(qh, dyn["len"], 1, rope_theta=cfg.rope_theta, rope=self.rotary)
             else:
                 import torch.distributed as dist
                 rank, world = self.sp
@@ -275,7 +306,7 @@ class DecoderStage:
             q, k, v = qkv.float().split((cfg.hidden, cfg.kv_hidden, cfg.kv_hidden))
             q = self._rope_q(q.view(H, HEAD_DIM), pos).contiguous()
             c.append(k.contiguous(), v.contiguous())
-            o = c.attend(q, rope_theta=cfg.rope_theta)
+            o = c.attend(q, rope_theta=cfg.rope_theta, rope=self.rotary)
             x = x + ly.wo @ o.half().view(-1)
             gu = ly.wgu @ rmsnorm(x, ly.n2, cfg.rms_eps)
             g, u = gu.split(cfg.intermediate)
@@ -325,7 +356,7 @@ class DecoderStage:
                 pos = c.n_sink + c.pos_base + c.len + torch.arange(n, device=self.device)
                 q = self._rope_rows(q.reshape(n, H, HEAD_DIM), pos).contiguous()
                 k, v = k.contiguous(), v.contiguous()
-                o = c.attend_chunk(q, k, v, rope_theta=cfg.rope_theta)
+                o = c.attend_chunk(q, k, v, rope_theta=cfg.rope_theta, rope=self.rotary)
                 c.append_chunk(k, v)
                 h = h + o.half().view(n, hid) @ ly.wo.t()
                 gu = rmsnorm(h, ly.n2, cfg.rms_eps) @ ly.wgu.t()
@@ -339,6 +370,8 @@ class DecoderStage:
         ang = pos.float()[:, None] * self.inv_freq[None, :]
         cos = torch.cat((ang.cos(), ang.cos()), dim=-1)[:, None, :]
         sin = torch.cat((ang.sin(), ang.sin()), dim=-1)[:, None, :]
+        if self.rotary is not None:
+            cos, sin = cos * self.rotary.attention_factor, sin * self.rotary.attention_factor
         rot = torch.cat((-q[..., self._half:], q[..., :self._half]), dim=-1)
         return q * cos + rot * sin
 
@@ -369,6 +402,8 @@ class GraphedStage:
         `recv from r-1 -> its layers -> send to (r+1) % world`, rank 0 additionally owns a second graph
         `recv from world-1 -> norm + lm_head`.  NCCL send/recv kernels inside the graph cost microseconds per hop; issued
         from the host every hop pays the launch latency of a host-issued collective."""
+        if pp is not None and pp[1] > 1 and stage.rotary is not None:
+            raise NotImplementedError("a layer-pipelined step with scaled rotary frequencies")
         self.stage = stage
         self.pp = pp
         dev = stage.device
@@ -579,11 +614,18 @@ class BatchedDecoderStage:
         hid = cfg.hidden
         for ly, bc in zip(self.stage.layers, self.caches):
             qkv = (rmsnorm(x, ly.n1, cfg.rms_eps) @ ly.wqkv.t()).contiguous()
-            _lib.check(lib.kvq_dec_rope_split_batch(qkv.data_ptr(), self.stage.inv_freq.data_ptr(), self.lens.data_ptr(),
-                                                    bc.n_sink, self._q.data_ptr(), self._k.data_ptr(), self._v.data_ptr(),
-                                                    cfg.n_heads, cfg.kv_heads, B, st), "kvq_dec_rope_split_batch")
+            rot = self.stage.rotary
+            if rot is None:
+                _lib.check(lib.kvq_dec_rope_split_batch(
+                    qkv.data_ptr(), self.stage.inv_freq.data_ptr(), self.lens.data_ptr(), bc.n_sink, self._q.data_ptr(),
+                    self._k.data_ptr(), self._v.data_ptr(), cfg.n_heads, cfg.kv_heads, B, st), "kvq_dec_rope_split_batch")
+            else:
+                _lib.check(lib.kvq_dec_rope_split_freq(
+                    qkv.data_ptr(), self.stage.inv_freq.data_ptr(), rot.attention_factor, self.lens.data_ptr(),
+                    bc.n_sink, self._q.data_ptr(), self._k.data_ptr(), self._v.data_ptr(), cfg.n_heads, cfg.kv_heads, B,
+                    st), "kvq_dec_rope_split_freq")
             bc.append_dyn(self._k, self._v, active=self.active)
-            o = bc.attend(self._q, out=self._o, len_add=1, rope_theta=cfg.rope_theta)
+            o = bc.attend(self._q, out=self._o, len_add=1, rope_theta=cfg.rope_theta, rope=rot)
             x = x + o.half().view(B, hid) @ ly.wo.t()
             gu = rmsnorm(x, ly.n2, cfg.rms_eps) @ ly.wgu.t()
             g, u = gu.split(cfg.intermediate, dim=-1)

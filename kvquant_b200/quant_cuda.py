@@ -18,9 +18,11 @@ from __future__ import annotations
 import torch
 
 from . import _lib
+from .rope import RotarySpec
 
 _HEAD_DIM = 128
-_rope_tables = {}  # (device index, theta) -> (f32 [64, npos, 2], half2 [64, npos] as int32, npos, build event)
+_rope_tables = {}  # (device index, theta or RotarySpec.key) -> (f32 [64, npos, 2], half2 [64, npos] as int32, npos, build event)
+_rope_freqs = {}   # (device index, RotarySpec.key) -> f32 [64] inv_freq on the device (read by the freq table builders)
 _rope_retired = []  # superseded tables stay allocated (graphs / other streams may still read them)
 
 
@@ -57,28 +59,54 @@ def _cache_dims(mat, bits):
     return H, Lmax
 
 
-def rope_tables(device, theta: float, min_npos: int):
+def rope_freq(device, spec):
+    """HF's inv_freq of a scaled RotarySpec as a device f32 [64] tensor (one per device and spec, never freed: the
+    attend entry points and captured graphs hold its pointer)."""
+    dev = device.index if device.index is not None else torch.cuda.current_device()
+    f = _rope_freqs.get((dev, spec.key))
+    if f is None:
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("rope frequencies of %r must be on the device before graph capture" % (spec,))
+        f = spec.inv_freq.to(torch.device("cuda", dev))
+        _rope_freqs[(dev, spec.key)] = f
+    return f
+
+
+def rope_tables(device, theta, min_npos: int):
     """(f32 table [64, npos, 2], half2 table [64, npos] as int32, npos) with npos >= min_npos; grown geometrically.
 
+    theta: the rope base (float), or a scaled kvquant_b200.rope.RotarySpec, whose tables are built from its frequency
+    vector and attention factor (kvq_rope_table_build_freq[_half]).
     Superseded tables are never freed: a captured CUDA graph (or a kernel still in flight on another stream) may hold
     their raw pointers.  Both tables are built on the current stream; an event recorded after the build is waited on
     by every later caller's stream, so a consumer on another stream never reads a half-built table."""
     dev = device.index if device.index is not None else torch.cuda.current_device()
-    key = (dev, float(theta))
+    spec = theta if isinstance(theta, RotarySpec) else None
+    if spec is not None and not spec.scaled:
+        spec, theta = None, spec.theta
+    key = (dev, spec.key) if spec is not None else (dev, float(theta))
     cur = _rope_tables.get(key)
     if cur is None or cur[2] < min_npos:
         npos = max(int(min_npos), 2 * cur[2] if cur else 0, 4096)
         npos = (npos + 255) // 256 * 256
         if torch.cuda.is_current_stream_capturing():
-            raise RuntimeError("rope table for theta=%g must cover %d positions before graph capture "
-                               "(call rope_tables() once outside the capture)" % (theta, min_npos))
+            raise RuntimeError("rope table for %s must cover %d positions before graph capture "
+                               "(call rope_tables() once outside the capture)"
+                               % (spec if spec is not None else "theta=%g" % theta, min_npos))
         t = torch.empty((64, npos, 2), dtype=torch.float32, device=device)
         th = torch.empty((64, npos), dtype=torch.int32, device=device)
         lib = _lib.load()
         with torch.cuda.device(device):
-            _lib.check(lib.kvq_rope_table_build(t.data_ptr(), float(theta), npos, _stream()), "kvq_rope_table_build")
-            _lib.check(lib.kvq_rope_table_build_half(th.data_ptr(), float(theta), npos, _stream()),
-                       "kvq_rope_table_build_half")
+            if spec is not None:
+                f, a = rope_freq(device, spec).data_ptr(), float(spec.attention_factor)
+                _lib.check(lib.kvq_rope_table_build_freq(t.data_ptr(), f, a, npos, _stream()),
+                           "kvq_rope_table_build_freq")
+                _lib.check(lib.kvq_rope_table_build_freq_half(th.data_ptr(), f, a, npos, _stream()),
+                           "kvq_rope_table_build_freq_half")
+            else:
+                _lib.check(lib.kvq_rope_table_build(t.data_ptr(), float(theta), npos, _stream()), "kvq_rope_table_build")
+                _lib.check(lib.kvq_rope_table_build_half(th.data_ptr(), float(theta), npos, _stream()),
+                           "kvq_rope_table_build_half")
             ev = torch.cuda.Event()
             ev.record(torch.cuda.current_stream())
         if cur is not None:
