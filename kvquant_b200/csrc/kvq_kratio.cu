@@ -278,13 +278,14 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
   }
 
   const uint64_t pol_keep = policy_evict_last();
-  const uint32_t tab0 = smem_u32(s_tab);
+  uint32_t tab0 = smem_u32(s_tab);
   const int tl = lane & 15;
   KRHalf hs;
   hs.half = (uint32_t)lane >> 4;
   hs.rot = hs.half ? 30u : 2u;
   hs.bias = hs.half * (BITS == 4 ? 0x40404040u : (BITS == 2 ? 0x10101010u : 0x20u));
-  const uint32_t rat0 = smem_u32(s_rat) + hs.half * 32u;
+  uint32_t rat0 = smem_u32(s_rat) + hs.half * 32u;
+  asm volatile("" : "+r"(tab0), "+r"(rat0));   // kept in registers, not rebuilt from the shared window every head
   mbar_wait(s_tabbar, 0);
   int s = 0;
   uint32_t ph = 0;
@@ -299,10 +300,15 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
     const bool mine = t < t_limit;
     float2 cs[32];
     if (warp / nlive < nh) {
-      const float2* rp = p.rope + (mine ? (t + p.pos_offset) : 0) + (int64_t)hs.half * p.rope_npos;
+      // a lane past the range loads the range's last token's factors (its score is dropped at the store and the max)
+      const float2* rp = p.rope + ((mine ? t : t_limit - 1) + p.pos_offset) + (int64_t)hs.half * p.rope_npos;
+      // pair k sits 2k rows below pair 0 (channel 8 (k/4) + 2 (k%4) + half = 2k + half).  The row step is passed
+      // through an empty asm so that the 32 row offsets are walked per round: hoisted out of the round loop they are
+      // 64 live registers, which ptxas spills to the stack and reloads every round.
+      int64_t step = 2 * p.rope_npos;
+      asm volatile("" : "+l"(step));
 #pragma unroll
-      for (int k = 0; k < 32; ++k)      // pair of register k: channel 8 (k/4) + 2 (k%4) + half
-        cs[k] = mine ? ld_keep_f2(rp + (int64_t)(8 * (k >> 2) + 2 * (k & 3)) * p.rope_npos, pol_keep) : make_float2(0.f, 0.f);
+      for (int k = 0; k < 32; ++k, rp += step) cs[k] = ld_keep_f2(rp, pol_keep);
     }
     const int m = (kKRWarps - 1 - c) / nlive + 1;
     int next_h = warp / nlive;                           // this warp's next head (warp-uniform)
