@@ -96,6 +96,27 @@ KVQ_API int kvq_rope_table_build_freq(float* rope_cos_sin, const float* freq, fl
                                       void* stream);
 KVQ_API int kvq_rope_table_build_freq_half(void* rope_half, const float* freq, float attn_factor, int64_t n_pos,
                                            void* stream);
+/* Length-dependent rotary frequencies (HF rope_type "dynamic" and "longrope"; DESIGN.md section 4.14): the rotation
+ * state of B sequences, f_cur f32 [B, 64], state int64 [B, 2] and table float2 [B, 64, npos] (device; sequence b's
+ * table has the kvq_rope_table_build_freq layout).  One call is two launches: a prepare kernel (one CTA per sequence)
+ * finds s, writes f_cur[b] = f(s) and decides whether the table must change; then a rebuild kernel rewrites the positions
+ * the new frequencies cover, or exits at once.  s = s_host (len_dev NULL, B == 1) or pos_offset + min(max(len_dev[b] +
+ * len_add, 0), L_cap).  params: host double [2] = (theta, factor).
+ *   mode 0, dynamic NTK: s <= m_pos (max_position_embeddings): f_lo (HF's default inv_freq), table positions
+ *     [0, min(m_pos, npos)) built once; s > m_pos: f_j = (float)(1 / base'^(2j/128)) with base' = theta * (factor * s /
+ *     m_pos - (factor - 1))^(128/126) in double precision, positions [0, s) rebuilt whenever s changes.  f_hi unused.
+ *   mode 1, LongRoPE: f_lo (short factors) for s <= m_pos (original_max_position_embeddings), table [0, min(m_pos,
+ *     npos)); f_hi (long factors) above, table [0, npos).  Each built once per switch.
+ * Entries are (cosf(f_j p) * attn_factor, sinf(f_j p) * attn_factor): bit for bit kvq_rope_table_build_freq over f_cur.
+ * Set state to -1 for a table that holds nothing (a new or reset sequence).  The attend entry points read f_cur and the
+ * table as rope_freq and rope_cos_sin.  NULL pointers (f_hi with mode 1) -> KVQ_E_NULL; mode not 0 / 1, m_pos <= 0,
+ * npos outside [1, 2^30], B outside [1, 256], theta not finite or <= 1, factor (mode 0) not finite or <= 0, attn_factor
+ * not finite or <= 0, len_dev NULL with B != 1 or s outside [0, npos], or len_dev given with L_cap < 0, pos_offset < 0
+ * or pos_offset + L_cap > npos -> KVQ_E_SHAPE. */
+KVQ_API int kvq_rope_len_update(int mode, const double* params, int64_t m_pos, const float* f_lo, const float* f_hi,
+                                float attn_factor, int64_t s, const int64_t* len_dev, int64_t len_add, int64_t L_cap,
+                                int pos_offset, int B, float* f_cur, int64_t* state, float* table, int64_t npos,
+                                void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Legacy decode matvecs (results are ADDED to `mul`, which the caller pre-zeroes -- modeling_llama.py:782,1209).
@@ -339,6 +360,23 @@ KVQ_API int kvq_attend_paged_freq(int bits, int B, const float* q, const int32_t
                    int64_t rope_npos, const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
                    const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch, const void* rope_half,
                    void* stream, const int32_t* page_table, int max_pages, const int32_t* npages, int P);
+/* kvq_attend_batch_freq / kvq_attend_paged_freq with one table and frequency vector per sequence (length-dependent
+ * rotary, kvq_rope_len_update): rope_cos_sin float2 [B, 64, rope_npos], rope_freq f32 [B, 64]; sequence b reads its
+ * own.  Checks: the parent's, then rope_npos > 2^30 -> KVQ_E_SHAPE. */
+KVQ_API int kvq_attend_batch_freq_seq(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                   const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent,
+                   const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv,
+                   int64_t Lmax, int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
+                   int64_t rope_npos, const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                   const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch, const void* rope_half,
+                   void* stream);
+KVQ_API int kvq_attend_paged_freq_seq(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                   const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent,
+                   const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv,
+                   int n_pool, int64_t L_cap, const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin,
+                   int64_t rope_npos, const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                   const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch, const void* rope_half,
+                   void* stream, const int32_t* page_table, int max_pages, const int32_t* npages, int P);
 KVQ_API int kvq_page_copy(int bits, int H, int n_out, int P, int64_t s0, int64_t s1, const kvq_seq_ref* src,
                           const kvq_seq_ref* dst, void* stream);
 
@@ -554,6 +592,10 @@ KVQ_API int kvq_dec_rope_split_batch(const void* qkv_f16, const float* inv_freq,
 KVQ_API int kvq_dec_rope_split_freq(const void* qkv_f16, const float* inv_freq, float attn_factor,
                                     const int64_t* pos_dev, int64_t pos_add, float* q, float* k, float* v, int Hq,
                                     int Hkv, int B, void* stream);
+/* kvq_dec_rope_split_freq with row b rotated by inv_freq[b] (f32 [B, 64]: the f_cur of kvq_rope_len_update). */
+KVQ_API int kvq_dec_rope_split_freq_seq(const void* qkv_f16, const float* inv_freq, float attn_factor,
+                                        const int64_t* pos_dev, int64_t pos_add, float* q, float* k, float* v, int Hq,
+                                        int Hkv, int B, void* stream);
 KVQ_API int kvq_dec_counter_add_batch(int64_t* counter, const int32_t* active, int64_t delta, int B, void* stream);
 KVQ_API int kvq_dec_silu_mul(const void* gu_f16, void* act_f16, int n, void* stream);
 KVQ_API int kvq_dec_f32_to_f16(const float* a, void* b_f16, int n, void* stream);

@@ -30,6 +30,8 @@ SIGNATURES = {
     "kvq_rope_table_build_half": (_c_int, [_p, _c_f, _c_i64, _p]),
     "kvq_rope_table_build_freq": (_c_int, [_p, _p, _c_f, _c_i64, _p]),
     "kvq_rope_table_build_freq_half": (_c_int, [_p, _p, _c_f, _c_i64, _p]),
+    "kvq_rope_len_update": (_c_int, [_c_int, _p, _c_i64, _p, _p, _c_f, _c_i64, _p, _c_i64, _c_i64, _c_int, _c_int,
+                                     _p, _p, _p, _c_i64, _p]),
     "kvq_k_matvec": (_c_int, [_c_int, _p, _p, _p, _p, _c_int, _c_int, _c_i64, _c_i64, _p, _p, _c_int, _p, _c_i64,
                               _c_f, _c_int, _p]),
     "kvq_v_matvec": (_c_int, [_c_int, _p, _p, _p, _p, _c_int, _c_int, _c_i64, _c_i64, _p, _p, _c_int, _p]),
@@ -63,6 +65,12 @@ SIGNATURES = {
     "kvq_attend_paged_freq": (_c_int, [_c_int, _c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int,
                                        _c_int, _c_int, _c_i64, _p, _c_i64, _p, _c_i64, _p, _c_f, _c_int, _p, _p,
                                        _c_int, _p, _p, _p, _p, _p, _p, _c_int, _p, _c_int]),
+    "kvq_attend_batch_freq_seq": (_c_int, [_c_int, _c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int,
+                                           _c_int, _c_i64, _c_i64, _p, _c_i64, _p, _c_i64, _p, _c_f, _c_int, _p, _p,
+                                           _c_int, _p, _p, _p, _p, _p]),
+    "kvq_attend_paged_freq_seq": (_c_int, [_c_int, _c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _c_int,
+                                           _c_int, _c_int, _c_i64, _p, _c_i64, _p, _c_i64, _p, _c_f, _c_int, _p, _p,
+                                           _c_int, _p, _p, _p, _p, _p, _p, _c_int, _p, _c_int]),
     "kvq_page_copy": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_i64, _c_i64, _p, _p, _p]),
     "kvq_append_kv_fused": (_c_int, [_c_int, _c_int, _c_i64, _c_i64, _c_int, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                      _p, _p, _p, _p, _p, _p, _p]),
@@ -102,6 +110,7 @@ SIGNATURES = {
     "kvq_dec_counter_add": (_c_int, [_p, _c_i64, _p]),
     "kvq_dec_rope_split_batch": (_c_int, [_p, _p, _p, _c_i64, _p, _p, _p, _c_int, _c_int, _c_int, _p]),
     "kvq_dec_rope_split_freq": (_c_int, [_p, _p, _c_f, _p, _c_i64, _p, _p, _p, _c_int, _c_int, _c_int, _p]),
+    "kvq_dec_rope_split_freq_seq": (_c_int, [_p, _p, _c_f, _p, _c_i64, _p, _p, _p, _c_int, _c_int, _c_int, _p]),
     "kvq_dec_counter_add_batch": (_c_int, [_p, _p, _c_i64, _c_int, _p]),
     "kvq_dec_silu_mul": (_c_int, [_p, _p, _c_int, _p]),
     "kvq_dec_f32_to_f16": (_c_int, [_p, _p, _c_int, _p]),

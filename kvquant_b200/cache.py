@@ -19,7 +19,7 @@ import torch
 
 from . import _lib
 from . import quant_cuda as qc
-from .rope import RotarySpec, resolve as _resolve_rope
+from .rope import LengthDependentRotary, RotarySpec, resolve as _resolve_rope
 
 HEAD_DIM = 128
 
@@ -50,12 +50,74 @@ def build_k_lookup_table(upper, lower, centroids, num_heads, normscale=None, nor
 
 
 def _rope_call(device, rope):
-    """(entry point suffix, rotary arguments) of a fused attend over tables for `rope` (a float theta or a scaled
-    RotarySpec): the theta entry points take theta, their *_freq siblings the device frequency vector and the
-    attention factor in its place."""
+    """(entry point suffix, rotary arguments) of a fused attend over tables for `rope` (a float theta, a scaled
+    RotarySpec or a prepared RopeLenState): the theta entry points take theta, their *_freq siblings the device
+    frequency vector and the attention factor in its place."""
+    if isinstance(rope, RopeLenState):
+        return "_freq", (rope.f_cur.data_ptr(), float(rope.spec.attention_factor))
     if isinstance(rope, RotarySpec):
         return "_freq", (qc.rope_freq(device, rope).data_ptr(), float(rope.attention_factor))
     return "", (float(rope),)
+
+
+class RopeLenState:
+    """The device rotation state of B sequences under a LengthDependentRotary (kvq_rope_len_update, DESIGN.md section
+    4.14): the current frequencies f_cur f32 [B, 64], a table float2 [B, 64, npos] in the rope table layout, and a key
+    per sequence saying which frequencies its table holds.  update() prepares it for a call's s; the attend, dequantise
+    and chunk-attend methods take a prepared state as `rope=` and use it as is, so the layers of a decode step share
+    one state and prepare it once.  Its contents are a function of s alone: a sequence retired, refilled or forked
+    needs no reset."""
+
+    def __init__(self, spec, B, npos, device):
+        if not isinstance(spec, LengthDependentRotary):
+            raise TypeError("RopeLenState needs a LengthDependentRotary, got %r" % (type(spec).__name__,))
+        self.spec, self.B, self.device = spec, int(B), torch.device(device)
+        self.npos = (max(int(npos), 256) + 255) // 256 * 256
+        self.lib = _lib.load()
+        lo, hi = spec.base_vectors()
+        self.f_lo = lo.to(self.device)
+        self.f_hi = hi.to(self.device) if hi is not None else None
+        self.mode, params, self.m_pos = spec.device_params()
+        self._params = np.asarray(params, dtype=np.float64)      # read on the host by the call
+        self.f_cur = torch.empty((self.B, HEAD_DIM // 2), dtype=torch.float32, device=self.device)
+        self.state = torch.full((self.B, 2), -1, dtype=torch.int64, device=self.device)
+        self.table = torch.empty((self.B, HEAD_DIM // 2, self.npos, 2), dtype=torch.float32, device=self.device)
+
+    def fits(self, spec, B, npos):
+        return self.spec == spec and self.B == B and self.npos >= npos
+
+    def update(self, s=None, len_dev=None, len_add=0, L_cap=0, pos_offset=0):
+        """Prepare for one call: s (one sequence), or per sequence pos_offset + min(max(len_dev[b] + len_add, 0),
+        L_cap).  Two launches on the current stream, no allocation: can be captured."""
+        _lib.check(self.lib.kvq_rope_len_update(
+            self.mode, self._params.ctypes.data, self.m_pos, self.f_lo.data_ptr(),
+            self.f_hi.data_ptr() if self.f_hi is not None else None, float(self.spec.attention_factor),
+            int(s) if s is not None else 0, len_dev.data_ptr() if len_dev is not None else None, int(len_add),
+            int(L_cap), int(pos_offset), self.B, self.f_cur.data_ptr(), self.state.data_ptr(), self.table.data_ptr(),
+            self.npos, torch.cuda.current_stream().cuda_stream), "kvq_rope_len_update")
+        return self
+
+    def slot(self, b):
+        """Sequence b's state as a one-sequence state over the same memory."""
+        v = RopeLenState.__new__(RopeLenState)
+        v.__dict__.update(self.__dict__)
+        v.B = 1
+        v.f_cur, v.state, v.table = self.f_cur[b:b + 1], self.state[b:b + 1], self.table[b:b + 1]
+        return v
+
+
+def _resolve(rope, rope_theta):
+    """rope.resolve, with a prepared RopeLenState passed through as it is."""
+    return rope if isinstance(rope, RopeLenState) else _resolve_rope(rope, rope_theta)
+
+
+def _len_refusals(cache, spec):
+    """What a length-dependent rotation cannot serve (DESIGN.md section 4.14)."""
+    if cache.n_sink:
+        raise NotImplementedError("attention sinks with length-dependent rotary frequencies: the sink keys are stored "
+                                  "post-RoPE in fp16 and cannot be rotated again at another length's frequencies")
+    if getattr(cache, "precision", "fp32") == "fp16":
+        raise NotImplementedError("length-dependent rotary frequencies use the exact fp32 tables (precision='fp32')")
 
 
 def _on_cache_device(fn):
@@ -155,6 +217,8 @@ class LayerCache:
         self._scratch = None
         self._retired = []   # superseded scratch buffers (a captured graph may still point at them)
         self._out = torch.empty((self.Hq, HEAD_DIM), dtype=torch.float32, device=dev)
+        # RopeLenState under a LengthDependentRotary: created on first use, or set to share one (DecoderStage)
+        self.rope_len_state = None
         # lookup-table precision of the K side of the fused attend:
         #   "fp32" (default) exact: the one-wavefront "ratio" tables of kvq_kratio.cu, equal to the legacy op chain to ~1e-6;
         #   "fp16"           north_star's fp16 LUT (kvq_kfast.cu): ~20 % faster K kernel, output within 1e-3 of the exact
@@ -251,6 +315,28 @@ class LayerCache:
                 LayerCache._shared_scratch[self.device.index] = cur
         self._scratch = cur
 
+    def _len_rope(self, rope, **where):
+        """A float theta / RotarySpec as is; a LengthDependentRotary becomes this cache's RopeLenState prepared at
+        `where` (RopeLenState.update's arguments); a RopeLenState is used as the caller prepared it."""
+        if isinstance(rope, RopeLenState):
+            _len_refusals(self, rope.spec)
+            return rope
+        if not isinstance(rope, LengthDependentRotary):
+            return rope
+        _len_refusals(self, rope)
+        npos = self.Lmax + self.n_sink + self.pos_base + 1
+        st = self.rope_len_state
+        if st is None or not st.fits(rope, 1, npos):
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("the rotation state must be allocated before graph capture")
+            st = self.rope_len_state = RopeLenState(rope, 1, npos, self.device)
+        return st.update(**where)
+
+    @staticmethod
+    def _table(rope):
+        """(f32 table [64, npos, 2], npos) of a prepared one-sequence RopeLenState."""
+        return rope.table[0], rope.npos
+
     @_on_cache_device
     def append(self, k_new, v_new):
         """Quantise + pack + outlier split of one token's K and V, entirely on the device (one launch)."""
@@ -303,7 +389,8 @@ class LayerCache:
             # the per-token LUT rows hold the un-normed centroids while the outlier residuals were taken against the
             # Q-Norm table: the legacy-LUT V kernel would mix the two
             raise NotImplementedError("V Q-Norm needs the native V form (use_native_v=True)")
-        return self._attend(q, None, 0, _resolve_rope(rope, rope_theta), out, lse, self.len)
+        rope_theta = self._len_rope(_resolve(rope, rope_theta), s=self.n_sink + self.pos_base + self.len)
+        return self._attend(q, None, 0, rope_theta, out, lse, self.len)
 
     def _attend(self, q, len_dev, len_add, rope_theta, out, lse, L):
         """attend over L slots (len_dev None: kvq_attend_gqa) or attend_dyn with the cap L (kvq_attend_gqa_dyn).  With
@@ -311,7 +398,10 @@ class LayerCache:
         native, mha = self.use_native_v, self.group == 1
         self._ensure_scratch(self.lib.kvq_attend_scratch_bytes(self.Hq, max(L, 1)), 1.25 if len_dev is None else 1.0)
         pos_offset = self.n_sink + self.pos_base
-        rope, rope_h, npos = qc.rope_tables(self.device, rope_theta, L + pos_offset + 1)
+        if isinstance(rope_theta, RopeLenState):
+            (rope, npos), rope_h = self._table(rope_theta), None
+        else:
+            rope, rope_h, npos = qc.rope_tables(self.device, rope_theta, L + pos_offset + 1)
         fast = self.precision == "fp16" and native and mha
         out = self._out if out is None else out
         ns = self.n_sink if self.sink_k is not None else 0
@@ -355,8 +445,14 @@ class LayerCache:
             self._gqa_check()
         elif not self.use_native_v:
             raise NotImplementedError("device-resident length needs the native V form")
-        return self._attend(q, len_dev, len_add, _resolve_rope(rope, rope_theta), out, lse,
-                            self.Lmax if L_cap is None else int(L_cap))
+        L_cap = self.Lmax if L_cap is None else int(L_cap)
+        rope_theta = self._len_rope(_resolve(rope, rope_theta), len_dev=self._check_len_dev(len_dev),
+                                    len_add=len_add, L_cap=L_cap, pos_offset=self.n_sink + self.pos_base)
+        return self._attend(q, len_dev, len_add, rope_theta, out, lse, L_cap)
+
+    def _check_len_dev(self, len_dev):
+        self._vec(len_dev, 1, "len_dev", torch.int64)
+        return len_dev
 
     def _kv_out(self, t, n, name):
         """Caller-supplied fp16 [H, n, 128] output, possibly a view into a larger [H, S, 128] buffer: tokens and
@@ -394,8 +490,10 @@ class LayerCache:
                 self.vcache.data_ptr(), self.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._out_ptrs("v"),
                 self.n_out, rope.data_ptr() if rope is not None else None, npos, pos_offset,
                 ok, ov, stride, torch.cuda.current_stream().cuda_stream), "kvq_dequant_kv")
-        return self._dequantize(start, stop, self.len, self.pos_base, _resolve_rope(rope, rope_theta), out_k, out_v,
-                                call)
+        rope_theta = _resolve(rope, rope_theta)
+        if isinstance(rope_theta, (LengthDependentRotary, RopeLenState)) and (stop if stop is not None else self.len) > start:
+            rope_theta = self._len_rope(rope_theta, s=self.n_sink + self.pos_base + self.len)
+        return self._dequantize(start, stop, self.len, self.pos_base, rope_theta, out_k, out_v, call)
 
     def _dequantize(self, start, stop, n_cached, pos_base, rope_theta, out_k, out_v, call):
         """The body of dequantize for a cache of this one's shape holding n_cached tokens (this cache, or a slot of a
@@ -419,7 +517,9 @@ class LayerCache:
             return out_k, out_v
         pos_offset = self.n_sink + pos_base
         rope, npos = None, 0
-        if rope_theta is not None:
+        if isinstance(rope_theta, RopeLenState):
+            rope, npos = self._table(rope_theta)
+        elif rope_theta is not None:
             rope, _, npos = qc.rope_tables(self.device, rope_theta, stop + pos_offset)
 
         def run(ok, ov, stride):
@@ -449,7 +549,10 @@ class LayerCache:
         (views allowed): the chunk operands both chunk attentions use.  Returns the f32 rope table, covering
         p0 + T positions."""
         T = k.shape[0]
-        rope, _, _ = qc.rope_tables(self.device, rope_theta, p0 + T)
+        if isinstance(rope_theta, RopeLenState):
+            rope, _ = self._table(rope_theta)
+        else:
+            rope, _, _ = qc.rope_tables(self.device, rope_theta, p0 + T)
         cos, sin = rope[:, p0:p0 + T, 0].t()[:, None, :], rope[:, p0:p0 + T, 1].t()[:, None, :]   # [T, 1, 64]
         kc = k.view(T, self.H, HEAD_DIM)
         lo, hi = kc[..., :HEAD_DIM // 2], kc[..., HEAD_DIM // 2:]
@@ -477,8 +580,8 @@ class LayerCache:
         the spec's table in place of rope_theta's; q must be rotated with the same spec."""
         if self.group > 1:
             self._gqa_check()
-        self._chunk_check(q, k, v)
-        rope_theta = _resolve_rope(rope, rope_theta)
+        T = self._chunk_check(q, k, v)
+        rope_theta = self._len_rope(_resolve(rope, rope_theta), s=self.n_sink + self.pos_base + self.len + T)
         sinks = (self.sink_k, self.sink_v) if self.sink_k is not None else None
         return self._attend_chunk_sdpa(q, k, v, rope_theta, self.len, self.pos_base, sinks,
                                        lambda ok, ov: self.dequantize(0, self.len, rope_theta, out_k=ok, out_v=ov))
@@ -522,7 +625,7 @@ class LayerCache:
         if not self.use_native_v:
             raise NotImplementedError("attend_chunk_fused reads the native V form (use_native_v=True)")
         T = self._chunk_check(q, k, v)
-        rope_theta = _resolve_rope(rope, rope_theta)
+        rope_theta = self._len_rope(_resolve(rope, rope_theta), s=self.n_sink + self.pos_base + self.len + T)
         L = self.len
         ns = self.n_sink if self.sink_k is not None else 0
         pos_offset = self.n_sink + self.pos_base
@@ -569,6 +672,28 @@ class _BatchCommon:
         self._scratch = None
         self._retired = []
         self._out = torch.empty((B, self.Hq, HEAD_DIM), dtype=torch.float32, device=dev)
+        # RopeLenState of the B slots under a LengthDependentRotary: created on first use, or set to share one
+        # (BatchedDecoderStage)
+        self.rope_len_state = None
+
+    def _len_state(self, spec):
+        """The slots' RopeLenState for `spec` (allocated outside a capture; a sequence view of a contiguous batch
+        then rotates with its slot of it)."""
+        _len_refusals(self._tmpl, spec)
+        st = self.rope_len_state
+        if st is None or not st.fits(spec, self.B, self.Lmax + self.n_sink + 1):
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("the rotation state must be allocated before graph capture")
+            st = self.rope_len_state = RopeLenState(spec, self.B, self.Lmax + self.n_sink + 1, self.device)
+            for b, v in enumerate(getattr(self, "_views", ())):
+                v.rope_len_state = st.slot(b)
+        return st
+
+    def _len_slot(self, b, rope, s):
+        """Slot b's one-sequence state prepared at s, for a LengthDependentRotary; other rotations as they are."""
+        if isinstance(rope, LengthDependentRotary):
+            return self._len_state(rope).slot(b).update(s=s)
+        return rope
 
     @staticmethod
     def _check_batch(batch):
@@ -649,12 +774,19 @@ class _BatchCommon:
         past its length, so its output is meaningless and must be ignored.  rope (optional RotarySpec): the keys'
         rotary frequencies in place of rope_theta (kvq_attend_batch_freq / kvq_attend_paged_freq)."""
         c = self._tmpl
-        rope_theta = _resolve_rope(rope, rope_theta)
+        rope_theta = _resolve(rope, rope_theta)
         if c.precision == "fp16":
             raise NotImplementedError("the batched attend uses the exact fp32 K tables (precision='fp32')")
         L_cap = self.Lmax if L_cap is None else int(L_cap)
         if not 1 <= L_cap <= self.Lmax:
             raise ValueError("L_cap must be in [1, %d], got %d" % (self.Lmax, L_cap))
+        if isinstance(rope_theta, LengthDependentRotary):
+            rope_theta = self._len_state(rope_theta).update(len_dev=self.lens, len_add=len_add, L_cap=L_cap,
+                                                            pos_offset=self.n_sink)
+        elif isinstance(rope_theta, RopeLenState):
+            _len_refusals(c, rope_theta.spec)
+            if rope_theta.B != self.B:
+                raise ValueError("a RopeLenState of %d sequences for a batch of %d" % (rope_theta.B, self.B))
         need = self.lib.kvq_attend_batch_scratch_bytes(self.B, self.Hq, L_cap)
         if self._scratch is None or self._scratch.numel() < need:
             if torch.cuda.is_current_stream_capturing():
@@ -664,10 +796,15 @@ class _BatchCommon:
                 self._retired.append(self._scratch)
             self._scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
         pos_offset = self.n_sink
-        rope, _, npos = qc.rope_tables(self.device, rope_theta, L_cap + pos_offset + 1)
+        if isinstance(rope_theta, RopeLenState):   # one table and frequency vector per sequence
+            rope, npos = rope_theta.table, rope_theta.npos
+        else:
+            rope, _, npos = qc.rope_tables(self.device, rope_theta, L_cap + pos_offset + 1)
         out = self._out if out is None else out
         ns = self.n_sink if self.sink_k is not None else 0
         sfx, rargs = _rope_call(self.device, rope_theta)
+        if isinstance(rope_theta, RopeLenState):
+            sfx = "_freq_seq"
         args = (self.bits, self.B, self._rows(q, self.q_hidden, "q"), self.kcache.data_ptr(), c.klut_deq.data_ptr(),
                 *self._ptrs("k"), self.vcache.data_ptr(), c.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._ptrs("v"),
                 self.n_out, self.Hq, self.H, self._extent, L_cap, self.lens.data_ptr(), int(len_add), rope.data_ptr(),
@@ -1123,15 +1260,17 @@ class PagedLayerCache(_BatchCommon):
         fp16 K and V [H, stop - start, 128], the same values, with the same options (rope= included), outputs and
         checks."""
         b = self.pages._slot(b)
-        return self._dequantize_at(b, start, stop, self.pages.lens_host[b], _resolve_rope(rope, rope_theta), out_k,
-                                   out_v)
+        n = self.pages.lens_host[b]
+        rope_theta = self._len_slot(b, _resolve(rope, rope_theta), n + self.n_sink)
+        return self._dequantize_at(b, start, stop, n, rope_theta, out_k, out_v)
 
     @_on_cache_device
     def _attend_chunk_at(self, b, L, q, k, v, rope_theta):
         c = self._tmpl
         if c.group > 1:
             c._gqa_check()
-        c._chunk_check(q, k, v)
+        T = c._chunk_check(q, k, v)
+        rope_theta = self._len_slot(b, rope_theta, self.n_sink + L + T)
         sinks = (self.sink_k[b], self.sink_v[b]) if self.sink_k is not None else None
         return c._attend_chunk_sdpa(q, k, v, rope_theta, L, 0, sinks,
                                     lambda ok, ov: self._dequantize_at(b, 0, L, L, rope_theta, ok, ov))
@@ -1141,7 +1280,7 @@ class PagedLayerCache(_BatchCommon):
         tokens over its sinks, those tokens (dequantised in place, kvq_dequant_kv_paged) and the chunk; same arguments
         (rope= included), grouped-query rule and result, bit for bit.  The cache is not modified."""
         b = self.pages._slot(b)
-        return self._attend_chunk_at(b, self.pages.lens_host[b], q, k, v, _resolve_rope(rope, rope_theta))
+        return self._attend_chunk_at(b, self.pages.lens_host[b], q, k, v, _resolve(rope, rope_theta))
 
     def slot(self, b):
         """Slot b as the single-sequence cache DecoderStage.prefill(caches=...) drives (PagedSlot)."""
@@ -1164,7 +1303,7 @@ class PagedSlot:
         self.Lmax, self.n_sink = cache.Lmax, cache.n_sink
 
     def attend_chunk(self, q, k, v, rope_theta=10000.0, rope=None):
-        return self.cache._attend_chunk_at(self.b, self.len, q, k, v, _resolve_rope(rope, rope_theta))
+        return self.cache._attend_chunk_at(self.b, self.len, q, k, v, _resolve(rope, rope_theta))
 
     def append_chunk(self, k, v):
         self.len = self.cache._append_chunk_at(self.b, self.len, k, v)

@@ -195,6 +195,7 @@ static int attend_validate(const AttendCall& c) {
   if (bad_bits) return KVQ_E_BITS;
   if (c.freq && !c.rope_freq) return KVQ_E_NULL;
   if (c.freq && !(c.attn_factor > 0.f && c.attn_factor < INFINITY)) return KVQ_E_SHAPE;
+  if (c.rope_per_seq && (c.B < 1 || c.rope_npos > ((int64_t)1 << 30))) return KVQ_E_SHAPE;
   return 0;
 }
 
@@ -287,15 +288,20 @@ int kvq_attend_dyn(int bits, const float* q, const int32_t* kcache, const float*
 
 // The rotary side of a call: theta (the kvq_attend* entry points) or a frequency vector and attention factor (their
 // *_freq siblings), stored into the AttendCall by the shared bodies below.
+// The *_freq_seq entry points: one table and frequency vector per sequence of a batch (length-dependent rotary).
 struct RopeArg {
   float theta;
   const float* freq;
   float attn;
   bool scaled;
-  void set(AttendCall& c) const { c.theta = theta; c.freq = scaled; c.rope_freq = freq; c.attn_factor = attn; }
+  bool per_seq;
+  void set(AttendCall& c) const {
+    c.theta = theta; c.freq = scaled; c.rope_freq = freq; c.attn_factor = attn; c.rope_per_seq = per_seq;
+  }
 };
-static RopeArg theta_arg(float theta) { return RopeArg{theta, nullptr, 1.f, false}; }
-static RopeArg freq_arg(const float* freq, float attn) { return RopeArg{0.f, freq, attn, true}; }
+static RopeArg theta_arg(float theta) { return RopeArg{theta, nullptr, 1.f, false, false}; }
+static RopeArg freq_arg(const float* freq, float attn) { return RopeArg{0.f, freq, attn, true, false}; }
+static RopeArg freq_seq_arg(const float* freq, float attn) { return RopeArg{0.f, freq, attn, true, true}; }
 
 static int attend_gqa(int bits, const float* q, const int32_t* kcache, const float* klut, const float* k_outliers,
                       const int32_t* k_outlier_idx, const int32_t* vcache, const float* vlut_tok, const float* v_cent,
@@ -471,6 +477,29 @@ int kvq_attend_paged_freq(int bits, int B, const float* q, const int32_t* kcache
                           const void* rope_half, void* stream, const int32_t* page_table, int max_pages,
                           const int32_t* npages, int P) {
   return attend_paged(KVQ_BATCH_ARGS(n_pool, freq_arg(rope_freq, attn_factor)), page_table, max_pages, npages, P);
+}
+
+int kvq_attend_batch_freq_seq(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                              const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache,
+                              const float* v_cent, const float* v_aff, const float* v_outliers,
+                              const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int64_t Lmax, int64_t L_cap,
+                              const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin, int64_t rope_npos,
+                              const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                              const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
+                              const void* rope_half, void* stream) {
+  return attend_batch(KVQ_BATCH_ARGS(Lmax, freq_seq_arg(rope_freq, attn_factor)));
+}
+
+int kvq_attend_paged_freq_seq(int bits, int B, const float* q, const int32_t* kcache, const float* klut,
+                              const float* k_outliers, const int32_t* k_outlier_idx, const int32_t* vcache,
+                              const float* v_cent, const float* v_aff, const float* v_outliers,
+                              const int32_t* v_outlier_idx, int n_out, int Hq, int Hkv, int n_pool, int64_t L_cap,
+                              const int64_t* len_dev, int64_t len_add, const float* rope_cos_sin, int64_t rope_npos,
+                              const float* rope_freq, float attn_factor, int pos_offset, const void* sink_k,
+                              const void* sink_v, int n_sink, float* out, float* out_lse, void* scratch,
+                              const void* rope_half, void* stream, const int32_t* page_table, int max_pages,
+                              const int32_t* npages, int P) {
+  return attend_paged(KVQ_BATCH_ARGS(n_pool, freq_seq_arg(rope_freq, attn_factor)), page_table, max_pages, npages, P);
 }
 
 int kvq_attend_merge(const float* parts, int n_parts, int H, float* out, void* stream) {

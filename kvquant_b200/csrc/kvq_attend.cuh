@@ -42,6 +42,8 @@ struct AttendCall {
   bool freq;                         // the *_freq entry points: the table was built from rope_freq and attn_factor
   const float* rope_freq;            // f32 [64] (device): the outlier pass's rotary frequencies, theta unused
   float attn_factor;
+  bool rope_per_seq;                 // batched *_seq entry points: sequence b's table and rope_freq sit b * 64 * rope_npos
+                                     // entries and b * 64 floats after sequence 0's (length-dependent frequencies)
   int pos_offset;
   const void* sink_k;
   const void* sink_v;

@@ -85,13 +85,17 @@ __global__ void dec_rope_split_batch_kernel(const __half* __restrict__ qkv, cons
 }
 
 // scaled rotary frequencies (kvq_dec_rope_split_freq): row b rotated at pos_add (+ pos_dev[b] when given) with
-// cos / sin times attn -- HF's attention_factor, applied to the query as to the keys (rope_table_freq_kernel)
-__global__ void dec_rope_split_freq_kernel(const __half* __restrict__ qkv, const float* __restrict__ inv_freq, float attn,
-                                           float pos_add, const int64_t* __restrict__ pos_dev, float* __restrict__ q,
-                                           float* __restrict__ k, float* __restrict__ v, int hidden, int kv_hidden) {
+// cos / sin times attn -- HF's attention_factor, applied to the query as to the keys (rope_table_freq_kernel).
+// SEQ (kvq_dec_rope_split_freq_seq): row b's frequencies are inv_freq[b][64] (length-dependent rotary).
+template <bool SEQ>
+__device__ __forceinline__ void dec_rope_split_freq_body(const __half* __restrict__ qkv, const float* __restrict__ inv_freq,
+                                                         float attn, float pos_add, const int64_t* __restrict__ pos_dev,
+                                                         float* __restrict__ q, float* __restrict__ k,
+                                                         float* __restrict__ v, int hidden, int kv_hidden) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= hidden) return;
   const int64_t r = blockIdx.y;
+  if constexpr (SEQ) inv_freq += r * kHalf;
   qkv += r * (hidden + 2 * kv_hidden);
   q += r * hidden; k += r * kv_hidden; v += r * kv_hidden;
   const float pos = pos_dev != nullptr ? pos_add + (float)pos_dev[r] : pos_add;
@@ -108,6 +112,19 @@ __global__ void dec_rope_split_freq_kernel(const __half* __restrict__ qkv, const
     k[i] = __half2float(qkv[hidden + i]);
     v[i] = __half2float(qkv[hidden + kv_hidden + i]);
   }
+}
+
+__global__ void dec_rope_split_freq_kernel(const __half* __restrict__ qkv, const float* __restrict__ inv_freq, float attn,
+                                           float pos_add, const int64_t* __restrict__ pos_dev, float* __restrict__ q,
+                                           float* __restrict__ k, float* __restrict__ v, int hidden, int kv_hidden) {
+  dec_rope_split_freq_body<false>(qkv, inv_freq, attn, pos_add, pos_dev, q, k, v, hidden, kv_hidden);
+}
+
+__global__ void dec_rope_split_freq_seq_kernel(const __half* __restrict__ qkv, const float* __restrict__ inv_freq,
+                                               float attn, float pos_add, const int64_t* __restrict__ pos_dev,
+                                               float* __restrict__ q, float* __restrict__ k, float* __restrict__ v,
+                                               int hidden, int kv_hidden) {
+  dec_rope_split_freq_body<true>(qkv, inv_freq, attn, pos_add, pos_dev, q, k, v, hidden, kv_hidden);
 }
 
 // counter[b] += delta for every b with active[b] != 0 (active == null: every b)
@@ -207,6 +224,18 @@ int kvq_dec_rope_split_freq(const void* qkv_f16, const float* inv_freq, float at
   if (!(attn_factor > 0.f && attn_factor < INFINITY)) return KVQ_E_SHAPE;
   const int hidden = Hq * kHeadDim;
   dec_rope_split_freq_kernel<<<dim3((hidden + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const __half*>(qkv_f16), inv_freq, attn_factor, (float)pos_add, pos_dev, q, k, v, hidden, Hkv * kHeadDim);
+  KVQ_LAUNCH_CHECK();
+  return 0;
+}
+
+int kvq_dec_rope_split_freq_seq(const void* qkv_f16, const float* inv_freq, float attn_factor, const int64_t* pos_dev,
+                                int64_t pos_add, float* q, float* k, float* v, int Hq, int Hkv, int B, void* stream) {
+  if (!qkv_f16 || !inv_freq || !q || !k || !v) return KVQ_E_NULL;
+  if (check_split_gqa(Hq, Hkv) || B < 1 || B > 65535) return KVQ_E_SHAPE;
+  if (!(attn_factor > 0.f && attn_factor < INFINITY)) return KVQ_E_SHAPE;
+  const int hidden = Hq * kHeadDim;
+  dec_rope_split_freq_seq_kernel<<<dim3((hidden + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __half*>(qkv_f16), inv_freq, attn_factor, (float)pos_add, pos_dev, q, k, v, hidden, Hkv * kHeadDim);
   KVQ_LAUNCH_CHECK();
   return 0;

@@ -282,7 +282,9 @@ constexpr size_t kOutThetaBytes = kHalf * sizeof(float);   // dynamic shared mem
 // FREQ (k_outlier_pers_freq_kernel): scaled rotary frequencies (DESIGN.md section 4.13).  The computed factors use
 // f_j = rope_freq[j] in place of rope_row_theta(rope_theta, j), times attn, as rope_table_freq_kernel builds the table;
 // rope_freq == null gathers every factor from the table (the wrapper passes rope_theta = 1 or 0 for given or null).
-template <bool GQA, bool BATCH, bool PAGED, bool FREQ>
+// SEQ (with BATCH and FREQ; k_outlier_pers_seq_kernel): length-dependent frequencies (DESIGN.md section 4.14), a table
+// and a frequency vector per sequence: sequence b's are 64 * rope_npos entries and 64 floats after sequence b-1's.
+template <bool GQA, bool BATCH, bool PAGED, bool FREQ, bool SEQ = false>
 __device__ __forceinline__ void k_outlier_pers_body(
     const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
     float* __restrict__ out, int64_t stride_h, int64_t stride_t, int64_t L, int H, int n_out,
@@ -298,6 +300,10 @@ __device__ __forceinline__ void k_outlier_pers_body(
     outliers += b * b_rows; outlier_idx += b * b_rows;
     out += b * b_out;
     len_dev += b;
+    if constexpr (SEQ) {
+      rope += (int64_t)b * kHalf * rope_npos;
+      if (rope_freq != nullptr) rope_freq += b * kHalf;
+    }
   }
   if (len_dev != nullptr) {                              // device-resident length: L is the cap the grid was sized for
     const int64_t l = *len_dev + len_add;
@@ -435,6 +441,19 @@ __global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_freq_kernel(
                                                b_out, b_rows, pg, rope_freq, attn);
 }
 
+template <bool GQA, bool PAGED>
+__global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_seq_kernel(
+    const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
+    float* __restrict__ out, int64_t stride_h, int64_t stride_t, int64_t L, int H, int n_out,
+    const float2* __restrict__ rope, int64_t rope_npos, int pos_offset, float scale,
+    const int64_t* __restrict__ len_dev, int64_t len_add, const float* __restrict__ rope_freq, float attn, int grp,
+    const int64_t b_out, const int64_t b_rows, const PageRef pg) {
+  k_outlier_pers_body<GQA, true, PAGED, true, true>(q, outliers, outlier_idx, out, stride_h, stride_t, L, H, n_out, rope,
+                                                    rope_npos, pos_offset, scale, len_dev, len_add, nullptr,
+                                                    rope_freq != nullptr ? 1.f : 0.f, grp, b_out, b_rows, pg,
+                                                    rope_freq, attn);
+}
+
 static int k_out_impl_table() {   // KVQ_KOUT_IMPL=table selects the non-persistent gather form for A/B runs
   static int v = -1;
   if (v < 0) { const char* e = getenv("KVQ_KOUT_IMPL"); v = (e && e[0] == 't') ? 1 : 0; }
@@ -452,14 +471,17 @@ static bool k_out_direct(int64_t n_positions, bool half_table) {
   return n_positions > (thr >= 0 ? thr : (half_table ? 64 * 1024 : 0));
 }
 
-static int set_k_outlier_smem(size_t smem, bool gqa, bool batch, bool paged, bool freq = false) {
-  static size_t smem_set_dev[12][64];  // per kernel and device: largest dynamic shared memory opted in so far (0 = 48 KiB)
+static int set_k_outlier_smem(size_t smem, bool gqa, bool batch, bool paged, bool freq = false, bool seq = false) {
+  static size_t smem_set_dev[16][64];  // per kernel and device: largest dynamic shared memory opted in so far (0 = 48 KiB)
   int dev_idx = 0;
   cudaGetDevice(&dev_idx);
-  size_t& smem_set = smem_set_dev[gqa + 2 * (batch + paged) + 6 * freq][dev_idx & 63];
+  size_t& smem_set = smem_set_dev[seq ? 12 + gqa + 2 * paged : gqa + 2 * (batch + paged) + 6 * freq][dev_idx & 63];
   if (smem_set == 0) smem_set = 48 * 1024;
   if (smem > smem_set) {
     const cudaError_t e = with_flavour(gqa, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
+      if (seq)
+        return cudaFuncSetAttribute(k_outlier_pers_seq_kernel<GQA(), PAGED()>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)smem);
       return freq ? cudaFuncSetAttribute(k_outlier_pers_freq_kernel<GQA(), BATCH(), PAGED()>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
                   : cudaFuncSetAttribute(k_outlier_pers_kernel<GQA(), BATCH(), PAGED()>,
@@ -536,6 +558,60 @@ __global__ void rope_table_freq_kernel(void* __restrict__ out, const float* __re
     } else {
       static_cast<float2*>(out)[(int64_t)j * n_pos + pos64] = e;
     }
+  }
+}
+
+// Length-dependent rotary frequencies (kvq_rope_len_update, DESIGN.md section 4.14).  Per sequence b: f_cur [b][64],
+// st [b][2] = (key of the frequencies the table holds, positions the rebuild writes) and a table [b][64][npos] in the
+// rope table layout.  s = one plus the last query position: s_host, or pos_offset + min(max(len_dev[b] + len_add, 0),
+// L_cap).  Dynamic NTK (mode 0): s <= m_pos reads f_lo (the default vector, one key for the whole range); s > m_pos is
+// HF's formula in double precision, rounded once to fp32, and a key per length.  LongRoPE (mode 1): f_lo (short) up
+// to m_pos (original_max_position_embeddings), f_hi (long) above, one key each.  A rebuild writes the positions its key
+// covers: [0, s) for a per-length key, [0, m_pos) or [0, npos) for a range key.  grid = B, block = 64.
+constexpr int kRopeLenDynamic = 0;
+__global__ void rope_len_prepare_kernel(int mode, double theta, double factor, int64_t m_pos, const float* __restrict__ f_lo,
+                                        const float* __restrict__ f_hi, int64_t s_host, const int64_t* __restrict__ len_dev,
+                                        int64_t len_add, int64_t L_cap, int pos_offset, float* __restrict__ f_cur,
+                                        int64_t* __restrict__ st, int64_t npos) {
+  const int b = blockIdx.x, j = threadIdx.x;
+  int64_t s = s_host;
+  if (len_dev != nullptr) {
+    const int64_t l = len_dev[b] + len_add;
+    s = pos_offset + (l < 0 ? 0 : (l < L_cap ? l : L_cap));
+  }
+  const bool above = s > m_pos;
+  const bool per_len = mode == kRopeLenDynamic && above;
+  float f;
+  if (per_len) {   // base * ((factor * s / M) - (factor - 1)) ** (128 / 126), then 1 / base' ** (2j / 128)
+    const double base = theta * pow(factor * (double)s / (double)m_pos - (factor - 1.0), 128.0 / 126.0);
+    f = (float)(1.0 / pow(base, (double)(2 * j) / 128.0));
+  } else {
+    f = (above ? f_hi : f_lo)[j];
+  }
+  f_cur[(int64_t)b * kHalf + j] = f;
+  if (j == 0) {
+    const int64_t key = per_len ? s : (above ? 1 : 0);   // a per-length key is s > m_pos >= 1: never 0 or 1
+    const int64_t end = per_len ? s : (above ? npos : m_pos);
+    int64_t* sb = st + 2 * b;
+    const bool rebuild = sb[0] != key;
+    sb[0] = key;
+    sb[1] = rebuild ? (end < npos ? end : npos) : 0;
+  }
+}
+
+// positions [0, st[b][1]) of sequence b's table from f_cur[b] -- rope_table_freq_kernel<false>'s expressions, bit for
+// bit its entries; st[b][1] == 0 exits at once.  grid = (x, 64, B).
+__global__ void rope_len_rebuild_kernel(const float* __restrict__ f_cur, const int64_t* __restrict__ st, float attn,
+                                        float2* __restrict__ table, int64_t npos) {
+  const int j = blockIdx.y, b = blockIdx.z;
+  const int64_t n = st[2 * b + 1];
+  const int64_t p0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p0 >= n) return;
+  const float f = f_cur[(int64_t)b * kHalf + j];
+  float2* row = table + ((int64_t)b * kHalf + j) * npos;
+  for (int64_t pos64 = p0; pos64 < n; pos64 += (int64_t)gridDim.x * blockDim.x) {
+    const float2 cs = rope_cos_sin(f, (int)pos64);
+    row[pos64] = make_float2(cs.x * attn, cs.y * attn);
   }
 }
 
@@ -624,7 +700,7 @@ int k_scores_batch(const AttendCall& c, const AttendScratch& s) {
     k_batch_zero_kernel<<<dim3((unsigned)std::min<int64_t>((c.L + 2047) / 2048, 64), H, B), 256, 0, c.stream>>>(
         s.scores, s.stride, s.bstride, c.len_dev, c.len_add, c.L);
     KVQ_LAUNCH_CHECK();
-    const int rc = set_k_outlier_smem(smem + kOutThetaBytes, grp > 1, true, c.pg != nullptr, c.freq);
+    const int rc = set_k_outlier_smem(smem + kOutThetaBytes, grp > 1, true, c.pg != nullptr, c.freq, c.rope_per_seq);
     if (rc != 0) return rc;
     const dim3 grid(k_outlier_grid(c.L * c.n_out, smem, B), (unsigned)B);
     const bool direct = k_out_direct(c.L + c.pos_offset, false);
@@ -633,7 +709,11 @@ int k_scores_batch(const AttendCall& c, const AttendScratch& s) {
     const float2* rope = reinterpret_cast<const float2*>(c.rope);
     const PageRef pg = c.pg != nullptr ? *c.pg : PageRef{};
     with_flavour(grp > 1, true, c.pg != nullptr, [&](auto GQA, auto BATCH, auto PAGED) {
-      if (c.freq)
+      if (c.rope_per_seq)
+        k_outlier_pers_seq_kernel<GQA(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
+            c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, rope, c.rope_npos, c.pos_offset,
+            1.f, c.len_dev, c.len_add, direct ? c.rope_freq : nullptr, c.attn_factor, grp, s.bstride, b_rows, pg);
+      else if (c.freq)
         k_outlier_pers_freq_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
             c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, rope, c.rope_npos, c.pos_offset,
             1.f, c.len_dev, c.len_add, nullptr, direct ? c.rope_freq : nullptr, c.attn_factor, grp, s.bstride, b_rows, pg);
@@ -680,6 +760,27 @@ int kvq_rope_table_build_freq(float* rope_cos_sin, const float* freq, float attn
 
 int kvq_rope_table_build_freq_half(void* rope_half, const float* freq, float attn_factor, int64_t n_pos, void* stream) {
   return rope_table_freq_build(rope_half, freq, attn_factor, n_pos, stream, true);
+}
+
+int kvq_rope_len_update(int mode, const double* params, int64_t m_pos, const float* f_lo, const float* f_hi,
+                        float attn_factor, int64_t s, const int64_t* len_dev, int64_t len_add, int64_t L_cap,
+                        int pos_offset, int B, float* f_cur, int64_t* state, float* table, int64_t npos, void* stream) {
+  if (!params || !f_lo || !f_cur || !state || !table || (mode == 1 && !f_hi)) return KVQ_E_NULL;
+  if ((mode != 0 && mode != 1) || m_pos <= 0 || npos <= 0 || npos > (int64_t)1 << 30 || B < 1 || B > 256) return KVQ_E_SHAPE;
+  const double theta = params[0], factor = params[1];
+  if (!(theta > 1.0 && theta < INFINITY) || (mode == 0 && !(factor > 0.0 && factor < INFINITY))) return KVQ_E_SHAPE;
+  if (!(attn_factor > 0.f && attn_factor < INFINITY)) return KVQ_E_SHAPE;
+  if (len_dev == nullptr ? (B != 1 || s < 0 || s > npos) : (L_cap < 0 || pos_offset < 0 || pos_offset + L_cap > npos))
+    return KVQ_E_SHAPE;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  rope_len_prepare_kernel<<<B, kHalf, 0, st>>>(mode, theta, factor, m_pos, f_lo, f_hi, s, len_dev, len_add, L_cap,
+                                                pos_offset, f_cur, state, npos);
+  KVQ_LAUNCH_CHECK();
+  // a second launch: no rebuild CTA reads a sequence's decision while the prepare CTA writes it
+  const dim3 grid((unsigned)((npos + 255) / 256 > 16 ? 16 : (npos + 255) / 256), kHalf, (unsigned)B);
+  rope_len_rebuild_kernel<<<grid, 256, 0, st>>>(f_cur, state, attn_factor, reinterpret_cast<float2*>(table), npos);
+  KVQ_LAUNCH_CHECK();
+  return 0;
 }
 
 int kvq_k_matvec(int bits, const float* q, const int32_t* cache, float* mul, const float* lut, int B, int H,

@@ -26,8 +26,8 @@ from dataclasses import dataclass
 
 import torch
 
-from .cache import BatchedLayerCache, LayerCache, PagedLayerCache, PageTable, HEAD_DIM
-from .rope import RotarySpec
+from .cache import RopeLenState, BatchedLayerCache, LayerCache, PagedLayerCache, PageTable, HEAD_DIM
+from .rope import LengthDependentRotary, RotarySpec
 
 
 @dataclass
@@ -46,7 +46,9 @@ class DecodeConfig:
     sparse_v: bool = True      # False: outlier rows for K only (BASELINE configs[4]: capped K outliers)
     max_len: int = 4096        # quantised slots allocated per layer
     n_kv_heads: int = None     # grouped-query attention: KV heads (None: n_heads); query head h reads KV head h // g
-    rope_scaling: dict = None  # HF rope_scaling dict ("linear", "llama3", "yarn"); None: plain rope_theta frequencies
+    rope_scaling: dict = None  # HF rope_scaling dict ("linear", "llama3", "yarn", "dynamic", "longrope"); None: plain
+                               # rope_theta frequencies
+    max_position_embeddings: int = None   # HF's config value: the switch length of "dynamic" and LongRoPE's default factor
 
     @property
     def kv_heads(self):
@@ -58,7 +60,11 @@ class DecodeConfig:
 
     @property
     def rotary(self):
-        """The scaled RotarySpec of rope_theta + rope_scaling, or None for the plain-theta frequencies."""
+        """The scaled RotarySpec of rope_theta + rope_scaling, a LengthDependentRotary for "dynamic" and "longrope",
+        or None for the plain-theta frequencies."""
+        sc = self.rope_scaling or {}
+        if sc.get("rope_type", sc.get("type")) in ("dynamic", "longrope"):
+            return LengthDependentRotary(self.rope_theta, sc, self.max_position_embeddings)
         spec = RotarySpec(self.rope_theta, self.rope_scaling)
         return spec if spec.scaled else None
 
@@ -153,8 +159,16 @@ class DecoderStage:
             self.norm = torch.ones(cfg.hidden, dtype=torch.float16, device=self.device)
             self.lm_head = (torch.randn((cfg.vocab, cfg.hidden), generator=gen, device=self.device) * 0.02).half()
         half = HEAD_DIM // 2
+        self.rope_state = None
         if self.rotary is None:
             self.inv_freq = 1.0 / (cfg.rope_theta ** (torch.arange(0, HEAD_DIM, 2, device=self.device).float() / HEAD_DIM))
+        elif isinstance(self.rotary, LengthDependentRotary):
+            # one rotation state for every layer, prepared once per decode step (the host paths use inv_freq_at)
+            self.inv_freq = None
+            c0 = self.layers[0].cache
+            self.rope_state = RopeLenState(self.rotary, 1, c0.Lmax + c0.n_sink + c0.pos_base + 1, self.device)
+            for ly in self.layers:
+                ly.cache.rope_len_state = self.rope_state
         else:   # HF's inv_freq, the vector the caches' tables are built from
             self.inv_freq = self.rotary.inv_freq.to(self.device)
         self._half = half
@@ -168,9 +182,15 @@ class DecoderStage:
             return self._gemv(self.lm_head, x, 3, self._buffers()["logits"], norm_w=self.norm)
         return self.lm_head @ rmsnorm(x, self.norm, self.cfg.rms_eps)
 
+    def _inv_freq(self, s):
+        """The frequencies of a call whose last query sits at position s - 1."""
+        if isinstance(self.rotary, LengthDependentRotary):
+            return self.rotary.inv_freq_at(s).to(self.device)
+        return self.inv_freq
+
     def _rope_q(self, q, pos):
         """HF rotate-half RoPE on the query only (modeling_llama.py:1851-1859); q f32 [H,128]."""
-        ang = self.inv_freq * float(pos)
+        ang = self._inv_freq(int(pos) + 1) * float(pos)
         cos = torch.cat((ang.cos(), ang.cos()))
         sin = torch.cat((ang.sin(), ang.sin()))
         if self.rotary is not None:     # HF multiplies cos and sin by the attention factor (YaRN)
@@ -221,13 +241,22 @@ class DecoderStage:
         st = torch.cuda.current_stream().cuda_stream
         xs = (b["x0"], b["x1"])     # ping-pong residual stream (the caller's x is never written)
         flip = 0
+        rot, freq = self.rotary, self.inv_freq
+        if self.rope_state is not None:   # length-dependent: f(s) and the table, once for every layer of the step
+            c0 = self.layers[0].cache
+            if self.dyn is not None:
+                rot = self.rope_state.update(len_dev=self.dyn["len"], len_add=1, L_cap=c0.Lmax,
+                                             pos_offset=c0.n_sink + c0.pos_base)
+            else:
+                rot = self.rope_state.update(s=c0.n_sink + c0.pos_base + c0.len + 1)
+            freq = rot.f_cur
         for ly in self.layers:
             c = ly.cache
             dyn = self.dyn          # device-resident length / position (one graph for a growing cache) or None
             self._gemv(ly.wqkv, x, 3, b["qkv"], norm_w=ly.n1)
             if self.rotary is not None:   # (unsharded): position *pos_dev, or the host position
                 pos = (dyn["pos"].data_ptr(), 0) if dyn is not None else (None, c.n_sink + c.pos_base + c.len)
-                _lib.check(lib.kvq_dec_rope_split_freq(b["qkv"].data_ptr(), self.inv_freq.data_ptr(),
+                _lib.check(lib.kvq_dec_rope_split_freq(b["qkv"].data_ptr(), freq.data_ptr(),
                                                        self.rotary.attention_factor, *pos, b["q"].data_ptr(),
                                                        b["k"].data_ptr(), b["v"].data_ptr(), H, cfg.kv_heads, 1, st),
                            "kvq_dec_rope_split_freq")
@@ -247,10 +276,10 @@ class DecoderStage:
             if self.sp is None:
                 if dyn is None:
                     c.append(b["k"], b["v"])             # pre-RoPE K, per-token V: quantise + outlier split
-                    o = c.attend(qh, rope_theta=cfg.rope_theta, rope=self.rotary)   # f32 [H,128]
+                    o = c.attend(qh, rope_theta=cfg.rope_theta, rope=rot)   # f32 [H,128]
                 else:
                     c.append_dyn(b["k"], b["v"], dyn["len"])
-                    o = c.attend_dyn(qh, dyn["len"], 1, rope_theta=cfg.rope_theta, rope=self.rotary)
+                    o = c.attend_dyn(qh, dyn["len"], 1, rope_theta=cfg.rope_theta, rope=rot)
             else:
                 import torch.distributed as dist
                 rank, world = self.sp
@@ -367,7 +396,7 @@ class DecoderStage:
 
     def _rope_rows(self, q, pos):
         """_rope_q of every row: q f32 [n, H, 128] rotated at positions pos [n]."""
-        ang = pos.float()[:, None] * self.inv_freq[None, :]
+        ang = pos.float()[:, None] * self._inv_freq(int(pos[-1]) + 1)[None, :]
         cos = torch.cat((ang.cos(), ang.cos()), dim=-1)[:, None, :]
         sin = torch.cat((ang.sin(), ang.sin()), dim=-1)[:, None, :]
         if self.rotary is not None:
@@ -542,6 +571,13 @@ class BatchedDecoderStage:
                 bc.set_sinks(c.sink_k[None].expand(self.B, -1, -1, -1).contiguous(),
                              c.sink_v[None].expand(self.B, -1, -1, -1).contiguous())
             self.caches.append(bc)
+        self.rope_state = None
+        if isinstance(stage.rotary, LengthDependentRotary):   # one state per slot, shared by the layers
+            self.rope_state = self.caches[0]._len_state(stage.rotary)
+            for bc in self.caches[1:]:
+                bc.rope_len_state = self.rope_state
+                for b, v in enumerate(getattr(bc, "_views", ())):
+                    v.rope_len_state = self.rope_state.slot(b)
         # the layers attend one after another on one stream: one scratch serves them all
         scratch = torch.empty(self.caches[0].lib.kvq_attend_batch_scratch_bytes(self.B, cfg.n_heads, self.caches[0].Lmax),
                               dtype=torch.uint8, device=self.device)
@@ -612,10 +648,18 @@ class BatchedDecoderStage:
         lib = _lib.load()
         st = torch.cuda.current_stream().cuda_stream
         hid = cfg.hidden
+        rot = self.stage.rotary
+        if self.rope_state is not None:   # every slot's f(s) and table, once for every layer of the step
+            bc0 = self.caches[0]
+            rot = self.rope_state.update(len_dev=self.lens, len_add=1, L_cap=bc0.Lmax, pos_offset=bc0.n_sink)
         for ly, bc in zip(self.stage.layers, self.caches):
             qkv = (rmsnorm(x, ly.n1, cfg.rms_eps) @ ly.wqkv.t()).contiguous()
-            rot = self.stage.rotary
-            if rot is None:
+            if isinstance(rot, RopeLenState):
+                _lib.check(lib.kvq_dec_rope_split_freq_seq(
+                    qkv.data_ptr(), rot.f_cur.data_ptr(), rot.spec.attention_factor, self.lens.data_ptr(),
+                    bc.n_sink, self._q.data_ptr(), self._k.data_ptr(), self._v.data_ptr(), cfg.n_heads, cfg.kv_heads, B,
+                    st), "kvq_dec_rope_split_freq_seq")
+            elif rot is None:
                 _lib.check(lib.kvq_dec_rope_split_batch(
                     qkv.data_ptr(), self.stage.inv_freq.data_ptr(), self.lens.data_ptr(), bc.n_sink, self._q.data_ptr(),
                     self._k.data_ptr(), self._v.data_ptr(), cfg.n_heads, cfg.kv_heads, B, st), "kvq_dec_rope_split_batch")
