@@ -52,9 +52,10 @@ def build_k_lookup_table(upper, lower, centroids, num_heads, normscale=None, nor
 def _rope_call(device, rope):
     """(entry point suffix, rotary arguments) of a fused attend over tables for `rope` (a float theta, a scaled
     RotarySpec or a prepared RopeLenState): the theta entry points take theta, their *_freq siblings the device
-    frequency vector and the attention factor in its place."""
+    frequency vector and the attention factor in its place, and the batched *_freq_seq ones a vector and a table per
+    sequence (a RopeLenState of several sequences)."""
     if isinstance(rope, RopeLenState):
-        return "_freq", (rope.f_cur.data_ptr(), float(rope.spec.attention_factor))
+        return "_freq_seq" if rope.B > 1 else "_freq", (rope.f_cur.data_ptr(), float(rope.spec.attention_factor))
     if isinstance(rope, RotarySpec):
         return "_freq", (qc.rope_freq(device, rope).data_ptr(), float(rope.attention_factor))
     return "", (float(rope),)
@@ -803,8 +804,6 @@ class _BatchCommon:
         out = self._out if out is None else out
         ns = self.n_sink if self.sink_k is not None else 0
         sfx, rargs = _rope_call(self.device, rope_theta)
-        if isinstance(rope_theta, RopeLenState):
-            sfx = "_freq_seq"
         args = (self.bits, self.B, self._rows(q, self.q_hidden, "q"), self.kcache.data_ptr(), c.klut_deq.data_ptr(),
                 *self._ptrs("k"), self.vcache.data_ptr(), c.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._ptrs("v"),
                 self.n_out, self.Hq, self.H, self._extent, L_cap, self.lens.data_ptr(), int(len_add), rope.data_ptr(),

@@ -27,19 +27,29 @@ __global__ void __launch_bounds__(1024) dec_rmsnorm_kernel(const __half* __restr
     y[i] = __hmul(__float2half(__half2float(x[i]) * r), w[i]);
 }
 
-// qkv fp16 [hidden + 2*kv_hidden] -> q (HF rotate-half RoPE at `pos`, modeling_llama.py:1851-1859) f32 [hidden],
-// k, v f32 [kv_hidden] (kv_hidden < hidden: grouped-query attention)
-__global__ void dec_rope_split_kernel(const __half* __restrict__ qkv, const float* __restrict__ inv_freq, float pos,
-                                      const int64_t* __restrict__ pos_dev,
+// Row b = blockIdx.y of qkv fp16 [B][hidden + 2*kv_hidden] -> q (HF rotate-half RoPE at `pos`, modeling_llama.py:
+// 1851-1859) f32 [B][hidden], k, v f32 [B][kv_hidden] (kv_hidden < hidden: grouped-query attention).  pos = pos_add,
+// plus pos_dev[b] when given (device-resident positions: graph replays with a growing cache).  Row b turns at
+// inv_freq[b * f_stride + j] (f_stride 64: length-dependent frequencies, one vector per row; 0: one shared vector), and
+// cos / sin are times attn -- HF's attention_factor, applied to the query as to the keys (rope_table_kernel); attn = 1
+// for theta, where the product is exact.
+__global__ void dec_rope_split_kernel(const __half* __restrict__ qkv, const float* __restrict__ inv_freq, int f_stride,
+                                      float attn, float pos_add, const int64_t* __restrict__ pos_dev,
                                       float* __restrict__ q, float* __restrict__ k, float* __restrict__ v, int hidden,
                                       int kv_hidden) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= hidden) return;
-  if (pos_dev != nullptr) pos += (float)(*pos_dev);   // device-resident position (graph replays with a growing cache)
+  const int64_t r = blockIdx.y;
+  inv_freq += r * f_stride;
+  qkv += r * (hidden + 2 * kv_hidden);
+  q += r * hidden; k += r * kv_hidden; v += r * kv_hidden;
+  const float pos = pos_dev != nullptr ? pos_add + (float)pos_dev[r] : pos_add;
   const int c = i & (kHeadDim - 1), j = c & (kHalf - 1);
   const float ang = inv_freq[j] * pos;
   float sn, cs;
   sincosf(ang, &sn, &cs);
+  cs *= attn;
+  sn *= attn;
   const float a = __half2float(qkv[i]);
   const float b = __half2float(qkv[i ^ kHalf]);
   q[i] = a * cs + ((c < kHalf) ? -b : b) * sn;
@@ -59,73 +69,6 @@ __global__ void dec_silu_mul_kernel(const __half* __restrict__ gu, __half* __res
 }
 
 __global__ void dec_counter_add_kernel(int64_t* c, int64_t d) { *c += d; }
-
-// batched decode: row b of qkv fp16 [B][hidden + 2*kv_hidden] rotated at position pos_dev[b] + pos_add into row b of
-// q f32 [B][hidden], k, v f32 [B][kv_hidden] -- per row the arithmetic of dec_rope_split_kernel
-__global__ void dec_rope_split_batch_kernel(const __half* __restrict__ qkv, const float* __restrict__ inv_freq,
-                                            float pos_add, const int64_t* __restrict__ pos_dev, float* __restrict__ q,
-                                            float* __restrict__ k, float* __restrict__ v, int hidden, int kv_hidden) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= hidden) return;
-  const int64_t r = blockIdx.y;
-  qkv += r * (hidden + 2 * kv_hidden);
-  q += r * hidden; k += r * kv_hidden; v += r * kv_hidden;
-  const float pos = pos_add + (float)pos_dev[r];
-  const int c = i & (kHeadDim - 1), j = c & (kHalf - 1);
-  const float ang = inv_freq[j] * pos;
-  float sn, cs;
-  sincosf(ang, &sn, &cs);
-  const float a = __half2float(qkv[i]);
-  const float b = __half2float(qkv[i ^ kHalf]);
-  q[i] = a * cs + ((c < kHalf) ? -b : b) * sn;
-  if (i < kv_hidden) {
-    k[i] = __half2float(qkv[hidden + i]);
-    v[i] = __half2float(qkv[hidden + kv_hidden + i]);
-  }
-}
-
-// scaled rotary frequencies (kvq_dec_rope_split_freq): row b rotated at pos_add (+ pos_dev[b] when given) with
-// cos / sin times attn -- HF's attention_factor, applied to the query as to the keys (rope_table_freq_kernel).
-// SEQ (kvq_dec_rope_split_freq_seq): row b's frequencies are inv_freq[b][64] (length-dependent rotary).
-template <bool SEQ>
-__device__ __forceinline__ void dec_rope_split_freq_body(const __half* __restrict__ qkv, const float* __restrict__ inv_freq,
-                                                         float attn, float pos_add, const int64_t* __restrict__ pos_dev,
-                                                         float* __restrict__ q, float* __restrict__ k,
-                                                         float* __restrict__ v, int hidden, int kv_hidden) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= hidden) return;
-  const int64_t r = blockIdx.y;
-  if constexpr (SEQ) inv_freq += r * kHalf;
-  qkv += r * (hidden + 2 * kv_hidden);
-  q += r * hidden; k += r * kv_hidden; v += r * kv_hidden;
-  const float pos = pos_dev != nullptr ? pos_add + (float)pos_dev[r] : pos_add;
-  const int c = i & (kHeadDim - 1), j = c & (kHalf - 1);
-  const float ang = inv_freq[j] * pos;
-  float sn, cs;
-  sincosf(ang, &sn, &cs);
-  cs *= attn;
-  sn *= attn;
-  const float a = __half2float(qkv[i]);
-  const float b = __half2float(qkv[i ^ kHalf]);
-  q[i] = a * cs + ((c < kHalf) ? -b : b) * sn;
-  if (i < kv_hidden) {
-    k[i] = __half2float(qkv[hidden + i]);
-    v[i] = __half2float(qkv[hidden + kv_hidden + i]);
-  }
-}
-
-__global__ void dec_rope_split_freq_kernel(const __half* __restrict__ qkv, const float* __restrict__ inv_freq, float attn,
-                                           float pos_add, const int64_t* __restrict__ pos_dev, float* __restrict__ q,
-                                           float* __restrict__ k, float* __restrict__ v, int hidden, int kv_hidden) {
-  dec_rope_split_freq_body<false>(qkv, inv_freq, attn, pos_add, pos_dev, q, k, v, hidden, kv_hidden);
-}
-
-__global__ void dec_rope_split_freq_seq_kernel(const __half* __restrict__ qkv, const float* __restrict__ inv_freq,
-                                               float attn, float pos_add, const int64_t* __restrict__ pos_dev,
-                                               float* __restrict__ q, float* __restrict__ k, float* __restrict__ v,
-                                               int hidden, int kv_hidden) {
-  dec_rope_split_freq_body<true>(qkv, inv_freq, attn, pos_add, pos_dev, q, k, v, hidden, kv_hidden);
-}
 
 // counter[b] += delta for every b with active[b] != 0 (active == null: every b)
 __global__ void dec_counter_add_batch_kernel(int64_t* c, const int32_t* __restrict__ active, int64_t d, int B) {
@@ -153,50 +96,47 @@ int kvq_dec_rmsnorm(const void* x_f16, const void* w_f16, void* y_f16, int n, fl
   return 0;
 }
 
+static int check_split_gqa(int Hq, int Hkv) {
+  return (Hq <= 0 || Hkv <= 0 || Hq % Hkv != 0) ? KVQ_E_SHAPE : 0;
+}
+
+// the launch every kvq_dec_rope_split* entry point makes once its arguments are checked: B rows of Hq query heads
+static int dec_rope_split(const void* qkv_f16, const float* inv_freq, int f_stride, float attn, float pos_add,
+                          const int64_t* pos_dev, float* q, float* k, float* v, int Hq, int Hkv, int B, void* stream) {
+  const int hidden = Hq * kHeadDim;
+  dec_rope_split_kernel<<<dim3((hidden + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const __half*>(qkv_f16), inv_freq, f_stride, attn, pos_add, pos_dev, q, k, v, hidden, Hkv * kHeadDim);
+  KVQ_LAUNCH_CHECK();
+  return 0;
+}
+
 int kvq_dec_rope_split(const void* qkv_f16, const float* inv_freq, float pos, float* q, float* k, float* v, int hidden,
                        void* stream) {
   if (!qkv_f16 || !inv_freq || !q || !k || !v) return KVQ_E_NULL;
   if (hidden <= 0 || (hidden % kHeadDim) != 0) return KVQ_E_SHAPE;
-  dec_rope_split_kernel<<<(hidden + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __half*>(qkv_f16), inv_freq, pos, nullptr, q, k, v, hidden, hidden);
-  KVQ_LAUNCH_CHECK();
-  return 0;
+  return dec_rope_split(qkv_f16, inv_freq, 0, 1.f, pos, nullptr, q, k, v, hidden / kHeadDim, hidden / kHeadDim, 1, stream);
 }
 
 int kvq_dec_rope_split_dyn(const void* qkv_f16, const float* inv_freq, const int64_t* pos_dev, int64_t pos_add,
                            float* q, float* k, float* v, int hidden, void* stream) {
   if (!qkv_f16 || !inv_freq || !pos_dev || !q || !k || !v) return KVQ_E_NULL;
   if (hidden <= 0 || (hidden % kHeadDim) != 0) return KVQ_E_SHAPE;
-  dec_rope_split_kernel<<<(hidden + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __half*>(qkv_f16), inv_freq, (float)pos_add, pos_dev, q, k, v, hidden, hidden);
-  KVQ_LAUNCH_CHECK();
-  return 0;
-}
-
-static int check_split_gqa(int Hq, int Hkv) {
-  return (Hq <= 0 || Hkv <= 0 || Hq % Hkv != 0) ? KVQ_E_SHAPE : 0;
+  return dec_rope_split(qkv_f16, inv_freq, 0, 1.f, (float)pos_add, pos_dev, q, k, v, hidden / kHeadDim, hidden / kHeadDim, 1,
+                        stream);
 }
 
 int kvq_dec_rope_split_gqa(const void* qkv_f16, const float* inv_freq, float pos, float* q, float* k, float* v, int Hq,
                            int Hkv, void* stream) {
   if (!qkv_f16 || !inv_freq || !q || !k || !v) return KVQ_E_NULL;
   if (check_split_gqa(Hq, Hkv)) return KVQ_E_SHAPE;
-  const int hidden = Hq * kHeadDim;
-  dec_rope_split_kernel<<<(hidden + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __half*>(qkv_f16), inv_freq, pos, nullptr, q, k, v, hidden, Hkv * kHeadDim);
-  KVQ_LAUNCH_CHECK();
-  return 0;
+  return dec_rope_split(qkv_f16, inv_freq, 0, 1.f, pos, nullptr, q, k, v, Hq, Hkv, 1, stream);
 }
 
 int kvq_dec_rope_split_gqa_dyn(const void* qkv_f16, const float* inv_freq, const int64_t* pos_dev, int64_t pos_add,
                                float* q, float* k, float* v, int Hq, int Hkv, void* stream) {
   if (!qkv_f16 || !inv_freq || !pos_dev || !q || !k || !v) return KVQ_E_NULL;
   if (check_split_gqa(Hq, Hkv)) return KVQ_E_SHAPE;
-  const int hidden = Hq * kHeadDim;
-  dec_rope_split_kernel<<<(hidden + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __half*>(qkv_f16), inv_freq, (float)pos_add, pos_dev, q, k, v, hidden, Hkv * kHeadDim);
-  KVQ_LAUNCH_CHECK();
-  return 0;
+  return dec_rope_split(qkv_f16, inv_freq, 0, 1.f, (float)pos_add, pos_dev, q, k, v, Hq, Hkv, 1, stream);
 }
 
 int kvq_dec_counter_add(int64_t* counter, int64_t delta, void* stream) {
@@ -210,11 +150,7 @@ int kvq_dec_rope_split_batch(const void* qkv_f16, const float* inv_freq, const i
                              float* q, float* k, float* v, int Hq, int Hkv, int B, void* stream) {
   if (!qkv_f16 || !inv_freq || !pos_dev || !q || !k || !v) return KVQ_E_NULL;
   if (check_split_gqa(Hq, Hkv) || B < 1 || B > 65535) return KVQ_E_SHAPE;
-  const int hidden = Hq * kHeadDim;
-  dec_rope_split_batch_kernel<<<dim3((hidden + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __half*>(qkv_f16), inv_freq, (float)pos_add, pos_dev, q, k, v, hidden, Hkv * kHeadDim);
-  KVQ_LAUNCH_CHECK();
-  return 0;
+  return dec_rope_split(qkv_f16, inv_freq, 0, 1.f, (float)pos_add, pos_dev, q, k, v, Hq, Hkv, B, stream);
 }
 
 int kvq_dec_rope_split_freq(const void* qkv_f16, const float* inv_freq, float attn_factor, const int64_t* pos_dev,
@@ -222,11 +158,7 @@ int kvq_dec_rope_split_freq(const void* qkv_f16, const float* inv_freq, float at
   if (!qkv_f16 || !inv_freq || !q || !k || !v) return KVQ_E_NULL;
   if (check_split_gqa(Hq, Hkv) || B < 1 || B > 65535) return KVQ_E_SHAPE;
   if (!(attn_factor > 0.f && attn_factor < INFINITY)) return KVQ_E_SHAPE;
-  const int hidden = Hq * kHeadDim;
-  dec_rope_split_freq_kernel<<<dim3((hidden + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __half*>(qkv_f16), inv_freq, attn_factor, (float)pos_add, pos_dev, q, k, v, hidden, Hkv * kHeadDim);
-  KVQ_LAUNCH_CHECK();
-  return 0;
+  return dec_rope_split(qkv_f16, inv_freq, 0, attn_factor, (float)pos_add, pos_dev, q, k, v, Hq, Hkv, B, stream);
 }
 
 int kvq_dec_rope_split_freq_seq(const void* qkv_f16, const float* inv_freq, float attn_factor, const int64_t* pos_dev,
@@ -234,11 +166,7 @@ int kvq_dec_rope_split_freq_seq(const void* qkv_f16, const float* inv_freq, floa
   if (!qkv_f16 || !inv_freq || !q || !k || !v) return KVQ_E_NULL;
   if (check_split_gqa(Hq, Hkv) || B < 1 || B > 65535) return KVQ_E_SHAPE;
   if (!(attn_factor > 0.f && attn_factor < INFINITY)) return KVQ_E_SHAPE;
-  const int hidden = Hq * kHeadDim;
-  dec_rope_split_freq_seq_kernel<<<dim3((hidden + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __half*>(qkv_f16), inv_freq, attn_factor, (float)pos_add, pos_dev, q, k, v, hidden, Hkv * kHeadDim);
-  KVQ_LAUNCH_CHECK();
-  return 0;
+  return dec_rope_split(qkv_f16, inv_freq, kHalf, attn_factor, (float)pos_add, pos_dev, q, k, v, Hq, Hkv, B, stream);
 }
 
 int kvq_dec_counter_add_batch(int64_t* counter, const int32_t* active, int64_t delta, int B, void* stream) {

@@ -356,19 +356,6 @@ __global__ void k_fast_prep_kernel(const float* __restrict__ q, const float* __r
   }
 }
 
-// half2 rope table: the reference's expressions (quant_cuda_kernel.cu:3081, 3123-3126), rounded once to fp16
-__global__ void rope_table_half_kernel(uint32_t* __restrict__ out, float rope_theta, int64_t n_pos) {
-  const int j = blockIdx.y;
-  const int headdim = kHeadDim;
-  const int headdim2 = headdim / 2;
-  const float theta = powf(rope_theta, (-2 * __int2float_rd(j % headdim2) / __int2float_rd(headdim)));
-  for (int64_t pos64 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos64 < n_pos; pos64 += (int64_t)gridDim.x * blockDim.x) {
-    const int pos = (int)pos64;
-    const __half2 e = __floats2half2_rn(cosf(theta * pos), sinf(theta * pos));
-    out[(int64_t)j * n_pos + pos64] = *reinterpret_cast<const uint32_t*>(&e);
-  }
-}
-
 template <int BITS>
 static int launch_k_fast(KFParams p, const float* q, const float* lut, uint32_t* qtab, const int32_t* cache,
                          cudaStream_t st) {
@@ -423,14 +410,3 @@ int k_fast_dispatch(const AttendCall& c, const AttendScratch& s, int accumulate)
 }
 
 }  // namespace kvq
-
-using namespace kvq;
-
-extern "C" int kvq_rope_table_build_half(void* rope_half, float theta, int64_t n_pos, void* stream) {
-  if (!rope_half) return KVQ_E_NULL;
-  if (n_pos <= 0 || n_pos > (int64_t)1 << 30) return KVQ_E_SHAPE;
-  const dim3 grid((unsigned)((n_pos + 255) / 256 > 4096 ? 4096 : (n_pos + 255) / 256), kHalf);
-  rope_table_half_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<uint32_t*>(rope_half), theta, n_pos);
-  KVQ_LAUNCH_CHECK();
-  return 0;
-}

@@ -186,11 +186,13 @@ __device__ __forceinline__ float k_ratio_head(const uint32_t st, const uint32_t 
 // 160, lies inside one page; the box's first token is below the sequence's length, so its page is mapped.  The
 // length is also capped at npages[b] * P.  A token's score is the same instruction sequence whatever the range, so
 // the scores equal the contiguous batch's bit for bit.  Other instantiations ignore `pg`.
-// SEQ (with BATCH; k_ratio_seq_kernel): length-dependent frequencies (DESIGN.md section 4.14), one rope table per
-// sequence, sequence b's 64 * rope_npos entries after sequence b-1's.
-template <int BITS, bool GQA, bool BATCH, bool PAGED, bool SEQ>
-__device__ __forceinline__ void k_ratio_body(const CUtensorMap& tmap, const KRParams& p, const int group,
-                                             const int64_t bstride, const PageRef& pg) {
+// With BATCH, sequence b's rope table sits b * rope_bstride entries after sequence 0's: 64 * rope_npos for a rotation
+// per sequence (length-dependent frequencies, DESIGN.md section 4.14), 0 for one table shared by the batch.  It is the
+// last kernel argument, not a KRParams field, so that every other argument keeps its parameter-bank offset.
+template <int BITS, bool GQA, bool BATCH, bool PAGED = false>
+__global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_constant__ CUtensorMap tmap, const KRParams p,
+                                                                const int group, const int64_t bstride, const PageRef pg,
+                                                                const int64_t rope_bstride) {
   using C = KRCfg<BITS>;
   constexpr int W = C::W;
   const int grp = GQA ? group : 1;
@@ -304,7 +306,7 @@ __device__ __forceinline__ void k_ratio_body(const CUtensorMap& tmap, const KRPa
     if (warp / nlive < nh) {
       // a lane past the range loads the range's last token's factors (its score is dropped at the store and the max)
       const float2* rope = p.rope;
-      if constexpr (SEQ) rope += (int64_t)bz * kHalf * p.rope_npos;
+      if constexpr (BATCH) rope += bz * rope_bstride;
       const float2* rp = rope + ((mine ? t : t_limit - 1) + p.pos_offset) + (int64_t)hs.half * p.rope_npos;
       // pair k sits 2k rows below pair 0 (channel 8 (k/4) + 2 (k%4) + half = 2k + half).  The row step is passed
       // through an empty asm so that the 32 row offsets are walked per round: hoisted out of the round loop they are
@@ -357,19 +359,6 @@ __device__ __forceinline__ void k_ratio_body(const CUtensorMap& tmap, const KRPa
   }
 }
 
-template <int BITS, bool GQA, bool BATCH, bool PAGED = false>
-__global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_constant__ CUtensorMap tmap, const KRParams p,
-                                                                const int group, const int64_t bstride, const PageRef pg) {
-  k_ratio_body<BITS, GQA, BATCH, PAGED, false>(tmap, p, group, bstride, pg);
-}
-
-template <int BITS, bool GQA, bool PAGED>
-__global__ void __launch_bounds__(kKRThreads, 1) k_ratio_seq_kernel(const __grid_constant__ CUtensorMap tmap,
-                                                                    const KRParams p, const int group,
-                                                                    const int64_t bstride, const PageRef pg) {
-  k_ratio_body<BITS, GQA, true, PAGED, true>(tmap, p, group, bstride, pg);
-}
-
 // table T[h][c][code] = LUT * qe_c and ratios r_c = s_c q_{c^64} / qe_c (qe = q, or +-1e-30 where q is exactly 0);
 // grid = H query heads, block = 128 (thread = channel).  GQA: query head h reads the LUT of KV head h / grp.
 // BATCH: sequence b = blockIdx.y, q [B][H][128], its tables and ratios `bstride` floats after sequence b-1's.
@@ -398,14 +387,13 @@ __global__ void k_ratio_prep_kernel(const float* __restrict__ q, const float* __
   qrat[(int64_t)h * kHeadDim + gi * 16 + half * 8 + xy * 4 + k] = sg * qb / qa;
 }
 
-template <int BITS, bool GQA, bool BATCH, bool PAGED, bool SEQ>
+template <int BITS, bool GQA, bool BATCH, bool PAGED>
 static int set_k_ratio_smem() {
   static PerDeviceOnce attr_once;
   bool& attr_done = attr_once.cur();
   if (!attr_done) {
-    cudaError_t e;
-    if constexpr (SEQ) e = cudaFuncSetAttribute(k_ratio_seq_kernel<BITS, GQA, PAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kKRSmemBudget);
-    else e = cudaFuncSetAttribute(k_ratio_kernel<BITS, GQA, BATCH, PAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kKRSmemBudget);
+    const cudaError_t e = cudaFuncSetAttribute(k_ratio_kernel<BITS, GQA, BATCH, PAGED>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kKRSmemBudget);
     if (e != cudaSuccess) return (int)e;
     attr_done = true;
   }
@@ -436,9 +424,8 @@ static int launch_k_ratio(KRParams p, const AttendCall& c, const AttendScratch& 
   if (S < 2) return KVQ_E_UNSUPPORTED;
   p.n_stages = S;
   const size_t smem = (size_t)tab_span + (size_t)S * C::kStage + 8u * (2 * S + 1) + 4u * p.G + 1024u;
-  const bool seq = c.rope_per_seq;
   int rc = with_flavour(gqa, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
-    return seq ? set_k_ratio_smem<BITS, GQA(), true, PAGED(), true>() : set_k_ratio_smem<BITS, GQA(), BATCH(), PAGED(), false>();
+    return set_k_ratio_smem<BITS, GQA(), BATCH(), PAGED()>();
   });
   if (rc != 0) return rc;
   CUtensorMap tmap;
@@ -457,13 +444,10 @@ static int launch_k_ratio(KRParams p, const AttendCall& c, const AttendScratch& 
   p.range = kr_range(p.L, max_splits);
   const int64_t splits = (p.L + p.range - 1) / p.range;
   const dim3 grid = batch ? dim3((unsigned)splits, (unsigned)groups, (unsigned)B) : dim3((unsigned)splits, (unsigned)groups);
+  const int64_t rope_bstride = c.rope_per_seq ? kHalf * p.rope_npos : 0;
   with_flavour(gqa, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
-    if (seq)
-      k_ratio_seq_kernel<BITS, GQA(), PAGED()><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, s.bstride,
-                                                                               paged ? *c.pg : PageRef{});
-    else
-      k_ratio_kernel<BITS, GQA(), BATCH(), PAGED()><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, s.bstride,
-                                                                                    paged ? *c.pg : PageRef{});
+    k_ratio_kernel<BITS, GQA(), BATCH(), PAGED()><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, s.bstride,
+                                                                                  paged ? *c.pg : PageRef{}, rope_bstride);
   });
   KVQ_LAUNCH_CHECK();
   return 0;

@@ -206,7 +206,9 @@ constexpr int kOutThreads = 256;
 
 // theta_j of rotary row j, and (cos, sin)(theta_j * pos): the reference's expressions (quant_cuda_kernel.cu:3081 and
 // 3123-3126).  The rope table is built from them and the outlier pass evaluates them, so both hold the same bits.
-__device__ __forceinline__ float rope_row_theta(float rope_theta, int j) {
+// rope_row_theta runs once per row, not per entry: out of line, its powf leaves the outlier pass's register allocation
+// alone (inlined, ptxas puts cosf / sinf's slow-path reduction buffer of the one-sequence MHA pass in local memory).
+__device__ __noinline__ float rope_row_theta(float rope_theta, int j) {
   const int headdim = kHeadDim;
   const int headdim2 = headdim / 2;
   return powf(rope_theta, (-2 * __int2float_rd(j % headdim2) / __int2float_rd(headdim)));
@@ -215,6 +217,12 @@ __device__ __forceinline__ float2 rope_cos_sin(float theta, int pos) {
   const float c = cosf(theta * pos);
   const float s = sinf(theta * pos);
   return make_float2(c, s);
+}
+// The frequency of rotary row j: f[j] for a frequency vector (scaled or length-dependent rotary), else theta_j of base
+// theta.  Every table entry and every factor the outlier pass computes is (cos, sin)(f_j * pos) * a of this value (a =
+// 1 for theta, where the product is exact), so the two hold the same bits.
+__device__ __forceinline__ float rotary_row_freq(float theta, const float* __restrict__ f, int j) {
+  return f != nullptr ? f[j] : rope_row_theta(theta, j);
 }
 
 // thread = one (token, outlier slot) entry.  cos/sin come from the RoPE table (bit-identical to the reference's
@@ -261,7 +269,7 @@ __global__ void __launch_bounds__(kOutThreads) k_outlier_kernel(
 // Persistent form (default).  ncu on the kernel above: load/store data path 75 % busy -- per ENTRY one scattered
 // 8-byte rope read plus TWO scattered reads of q.  Here CTAs are persistent and keep (q[c], q[c^64]) for all channels
 // in shared memory (one 8-byte shared read per entry instead of two scattered global ones); the rotary factors are
-// computed (rope_theta > 0, k_out_direct) or gathered from the table.
+// computed (direct, k_out_direct) or gathered from the table.
 // Alternatives considered (DESIGN.md section 4.1): a second, token-major copy of the rope table read with coalesced
 // row loads + shuffles instead of the gather (it loads rows for the zero-valued pads too and adds 8 shuffles per
 // entry); gathering every entry's rotary factors from the rope table (slower than computing them, even at 32K);
@@ -279,31 +287,30 @@ __global__ void __launch_bounds__(kOutThreads) k_outlier_kernel(
 constexpr int kOutPersThreads = 512;
 constexpr size_t kOutThetaBytes = kHalf * sizeof(float);   // dynamic shared memory past the q table: s_th
 //
-// FREQ (k_outlier_pers_freq_kernel): scaled rotary frequencies (DESIGN.md section 4.13).  The computed factors use
-// f_j = rope_freq[j] in place of rope_row_theta(rope_theta, j), times attn, as rope_table_freq_kernel builds the table;
-// rope_freq == null gathers every factor from the table (the wrapper passes rope_theta = 1 or 0 for given or null).
-// SEQ (with BATCH and FREQ; k_outlier_pers_seq_kernel): length-dependent frequencies (DESIGN.md section 4.14), a table
-// and a frequency vector per sequence: sequence b's are 64 * rope_npos entries and 64 floats after sequence b-1's.
-template <bool GQA, bool BATCH, bool PAGED, bool FREQ, bool SEQ = false>
-__device__ __forceinline__ void k_outlier_pers_body(
+// Rotary factors: rotary row j turns at f_j = rotary_row_freq(rope_theta, rope_freq, j) -- theta_j of rope_theta when
+// rope_freq is null, else rope_freq[j] (scaled or length-dependent frequencies, DESIGN.md sections 4.13, 4.14) -- and
+// the factors are (cos, sin)(f_j * pos) * attn (attn = 1 for theta), as rope_table_kernel builds the table.  direct:
+// the pass computes them (past CUDART_TRIG_PLOSS_F it gathers them); otherwise every factor comes from the table.
+// With BATCH, sequence b's table and frequency vector sit b * rope_bstride entries and b * freq_bstride floats after
+// sequence 0's: 64 * rope_npos and 64 for a rotation per sequence, 0 for one shared by the batch.
+template <bool GQA, bool BATCH, bool PAGED>
+__global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
     const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
     float* __restrict__ out, int64_t stride_h, int64_t stride_t, int64_t L, int H, int n_out,
     const float2* __restrict__ rope, int64_t rope_npos, int pos_offset, float scale,
-    const int64_t* __restrict__ len_dev, int64_t len_add, const uint32_t* __restrict__ rope_h, float rope_theta, int grp,
-    const int64_t b_out, const int64_t b_rows, const PageRef pg, const float* __restrict__ rope_freq, float attn) {
+    const int64_t* __restrict__ len_dev, int64_t len_add, const uint32_t* __restrict__ rope_h, float rope_theta,
+    const float* __restrict__ rope_freq, float attn, bool direct, int grp, const int64_t b_out, const int64_t b_rows,
+    const PageRef pg, const int64_t rope_bstride, const int freq_bstride) {
   extern __shared__ float2 s_qq[];                       // [H*128] = (q[c], q[c^64]), query heads
-  float* const s_th = reinterpret_cast<float*>(s_qq + H * kHeadDim);   // [64]: theta_j of rotary row j (direct)
-  const bool direct = rope_theta > 0.f;
+  float* const s_th = reinterpret_cast<float*>(s_qq + H * kHeadDim);   // [64]: f_j of rotary row j (direct)
   if constexpr (BATCH) {
     const int b = blockIdx.y;
     q += (int64_t)b * H * kHeadDim;
     outliers += b * b_rows; outlier_idx += b * b_rows;
     out += b * b_out;
     len_dev += b;
-    if constexpr (SEQ) {
-      rope += (int64_t)b * kHalf * rope_npos;
-      if (rope_freq != nullptr) rope_freq += b * kHalf;
-    }
+    rope += b * rope_bstride;
+    if (rope_freq != nullptr) rope_freq += b * freq_bstride;
   }
   if (len_dev != nullptr) {                              // device-resident length: L is the cap the grid was sized for
     const int64_t l = *len_dev + len_add;
@@ -316,11 +323,7 @@ __device__ __forceinline__ void k_outlier_pers_body(
   const uint32_t total = (uint32_t)(L * n_out);          // host checks L * n_out < 2^31
   const int tid = threadIdx.x, lane = tid & 31;
   for (int i = tid; i < H * kHeadDim; i += kOutPersThreads) s_qq[i] = make_float2(q[i], q[i ^ kHalf]);
-  if constexpr (FREQ) {
-    if (direct && tid < kHalf) s_th[tid] = rope_freq[tid];
-  } else {
-    if (direct && tid < kHalf) s_th[tid] = rope_row_theta(rope_theta, tid);
-  }
+  if (direct && tid < kHalf) s_th[tid] = rotary_row_freq(rope_theta, rope_freq, tid);
   __syncthreads();
   const uint32_t stride = gridDim.x * kOutPersThreads;
   // outlier rows are read once: evict them first, so that the score rows the atomics add into (just cleared) stay in L2
@@ -362,10 +365,8 @@ __device__ __forceinline__ void k_outlier_pers_body(
           const bool fast = th * pos <= CUDART_TRIG_PLOSS_F;
           if (fast) cs = rope_cos_sin(th, pos);
           else cs = ld_keep_f2(rope + (int64_t)j * rope_npos + pos, pol_keep);
-          if constexpr (FREQ) {   // the table's entries already carry attn (a product with 1 is exact)
-            const float m = fast ? attn : 1.f;
-            cs = make_float2(cs.x * m, cs.y * m);
-          }
+          const float m = fast ? attn : 1.f;   // the table's entries already carry attn (a product with 1 is exact)
+          cs = make_float2(cs.x * m, cs.y * m);
         } else if (rope_h != nullptr) {   // fp16 mode: the half2 table the dense kernel streams (half the bytes per gather)
           uint32_t u;
           asm volatile("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(u)
@@ -416,44 +417,6 @@ __device__ __forceinline__ void k_outlier_pers_body(
   }
 }
 
-template <bool GQA, bool BATCH, bool PAGED = false>
-__global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_kernel(
-    const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
-    float* __restrict__ out, int64_t stride_h, int64_t stride_t, int64_t L, int H, int n_out,
-    const float2* __restrict__ rope, int64_t rope_npos, int pos_offset, float scale,
-    const int64_t* __restrict__ len_dev, int64_t len_add, const uint32_t* __restrict__ rope_h, float rope_theta, int grp,
-    const int64_t b_out, const int64_t b_rows, const PageRef pg) {
-  k_outlier_pers_body<GQA, BATCH, PAGED, false>(q, outliers, outlier_idx, out, stride_h, stride_t, L, H, n_out, rope,
-                                                rope_npos, pos_offset, scale, len_dev, len_add, rope_h, rope_theta, grp,
-                                                b_out, b_rows, pg, nullptr, 1.f);
-}
-
-template <bool GQA, bool BATCH, bool PAGED = false>
-__global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_freq_kernel(
-    const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
-    float* __restrict__ out, int64_t stride_h, int64_t stride_t, int64_t L, int H, int n_out,
-    const float2* __restrict__ rope, int64_t rope_npos, int pos_offset, float scale,
-    const int64_t* __restrict__ len_dev, int64_t len_add, const uint32_t* __restrict__ rope_h,
-    const float* __restrict__ rope_freq, float attn, int grp, const int64_t b_out, const int64_t b_rows, const PageRef pg) {
-  k_outlier_pers_body<GQA, BATCH, PAGED, true>(q, outliers, outlier_idx, out, stride_h, stride_t, L, H, n_out, rope,
-                                               rope_npos, pos_offset, scale, len_dev, len_add, rope_h,
-                                               rope_freq != nullptr ? 1.f : 0.f, grp,
-                                               b_out, b_rows, pg, rope_freq, attn);
-}
-
-template <bool GQA, bool PAGED>
-__global__ void __launch_bounds__(kOutPersThreads) k_outlier_pers_seq_kernel(
-    const float* __restrict__ q, const float* __restrict__ outliers, const int32_t* __restrict__ outlier_idx,
-    float* __restrict__ out, int64_t stride_h, int64_t stride_t, int64_t L, int H, int n_out,
-    const float2* __restrict__ rope, int64_t rope_npos, int pos_offset, float scale,
-    const int64_t* __restrict__ len_dev, int64_t len_add, const float* __restrict__ rope_freq, float attn, int grp,
-    const int64_t b_out, const int64_t b_rows, const PageRef pg) {
-  k_outlier_pers_body<GQA, true, PAGED, true, true>(q, outliers, outlier_idx, out, stride_h, stride_t, L, H, n_out, rope,
-                                                    rope_npos, pos_offset, scale, len_dev, len_add, nullptr,
-                                                    rope_freq != nullptr ? 1.f : 0.f, grp, b_out, b_rows, pg,
-                                                    rope_freq, attn);
-}
-
 static int k_out_impl_table() {   // KVQ_KOUT_IMPL=table selects the non-persistent gather form for A/B runs
   static int v = -1;
   if (v < 0) { const char* e = getenv("KVQ_KOUT_IMPL"); v = (e && e[0] == 't') ? 1 : 0; }
@@ -471,21 +434,16 @@ static bool k_out_direct(int64_t n_positions, bool half_table) {
   return n_positions > (thr >= 0 ? thr : (half_table ? 64 * 1024 : 0));
 }
 
-static int set_k_outlier_smem(size_t smem, bool gqa, bool batch, bool paged, bool freq = false, bool seq = false) {
-  static size_t smem_set_dev[16][64];  // per kernel and device: largest dynamic shared memory opted in so far (0 = 48 KiB)
+static int set_k_outlier_smem(size_t smem, bool gqa, bool batch, bool paged) {
+  static size_t smem_set_dev[6][64];   // per kernel and device: largest dynamic shared memory opted in so far (0 = 48 KiB)
   int dev_idx = 0;
   cudaGetDevice(&dev_idx);
-  size_t& smem_set = smem_set_dev[seq ? 12 + gqa + 2 * paged : gqa + 2 * (batch + paged) + 6 * freq][dev_idx & 63];
+  size_t& smem_set = smem_set_dev[gqa + 2 * (batch + paged)][dev_idx & 63];
   if (smem_set == 0) smem_set = 48 * 1024;
   if (smem > smem_set) {
     const cudaError_t e = with_flavour(gqa, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
-      if (seq)
-        return cudaFuncSetAttribute(k_outlier_pers_seq_kernel<GQA(), PAGED()>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)smem);
-      return freq ? cudaFuncSetAttribute(k_outlier_pers_freq_kernel<GQA(), BATCH(), PAGED()>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                  : cudaFuncSetAttribute(k_outlier_pers_kernel<GQA(), BATCH(), PAGED()>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      return cudaFuncSetAttribute(k_outlier_pers_kernel<GQA(), BATCH(), PAGED()>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     });
     if (e != cudaSuccess) return (int)e;
     smem_set = smem;
@@ -516,49 +474,53 @@ static int launch_k_outliers(const KParams& p, cudaStream_t st) {
     KVQ_LAUNCH_CHECK();
     return 0;
   }
-  const int rc = set_k_outlier_smem(smem + kOutThetaBytes, gqa, false, false, p.freq);
+  const int rc = set_k_outlier_smem(smem + kOutThetaBytes, gqa, false, false);
   if (rc != 0) return rc;
   const unsigned grid = k_outlier_grid(total, smem, 1);
   const bool direct = k_out_direct(p.L + p.pos_offset, p.rope_h != nullptr);
-  const float direct_theta = direct ? p.theta : 0.f;
   with_flavour(gqa, false, false, [&](auto GQA, auto BATCH, auto PAGED) {
-    if (p.freq)
-      k_outlier_pers_freq_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, st>>>(
-          p.q, p.outliers, p.outlier_idx, p.out, p.out_stride, 1, p.L, p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset,
-          1.f, p.len_dev, p.len_add, p.rope_h, direct ? p.rope_freq : nullptr, p.attn, gqa ? p.grp : 1, 0, 0, PageRef{});
-    else
-      k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, st>>>(
-          p.q, p.outliers, p.outlier_idx, p.out, p.out_stride, 1, p.L, p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset, 1.f,
-          p.len_dev, p.len_add, p.rope_h, direct_theta, gqa ? p.grp : 1, 0, 0, PageRef{});
+    k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, st>>>(
+        p.q, p.outliers, p.outlier_idx, p.out, p.out_stride, 1, p.L, p.H, p.n_out, p.rope, p.rope_npos, p.pos_offset, 1.f,
+        p.len_dev, p.len_add, p.rope_h, p.theta, p.freq ? p.rope_freq : nullptr, p.freq ? p.attn : 1.f, direct,
+        gqa ? p.grp : 1, 0, 0, PageRef{}, 0, 0);
   });
   KVQ_LAUNCH_CHECK();
   return 0;
 }
 
-// rope table: rope_row_theta / rope_cos_sin once per (j, p)
-__global__ void rope_table_kernel(float2* __restrict__ out, float rope_theta, int64_t n_pos) {
-  const int j = blockIdx.y;
-  const float theta = rope_row_theta(rope_theta, j);
-  for (int64_t pos64 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos64 < n_pos; pos64 += (int64_t)gridDim.x * blockDim.x)
-    out[(int64_t)j * n_pos + pos64] = rope_cos_sin(theta, (int)pos64);
-}
-
-// scaled rope table: (cosf(f_j p) * attn, sinf(f_j p) * attn), f_j = freq[j] -- the factors k_outlier_pers_freq_kernel
-// computes.  HALF: the same values rounded once to fp16 (half2 entries).
+// rope table [B][64][n_pos]: entry (j, p) = (cosf(f_j p) * attn, sinf(f_j p) * attn), f_j = rotary_row_freq(theta, f, j)
+// -- the factors k_outlier_pers_kernel computes.  HALF: the same values rounded once to fp16 (half2 entries).
+// Sequence b = blockIdx.z: its table and f follow b * 64 * n_pos entries and b * 64 floats after sequence 0's.
+// st (the length-dependent rebuild, kvq_rope_len_update): sequence b writes positions [0, st[b][1]) of its table;
+// null: every position.  grid = (x, 64, B).
 template <bool HALF>
-__global__ void rope_table_freq_kernel(void* __restrict__ out, const float* __restrict__ freq, float attn, int64_t n_pos) {
-  const int j = blockIdx.y;
-  const float f = freq[j];
-  for (int64_t pos64 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos64 < n_pos; pos64 += (int64_t)gridDim.x * blockDim.x) {
-    const float2 cs = rope_cos_sin(f, (int)pos64);
+__global__ void rope_table_kernel(void* __restrict__ out, float theta, const float* __restrict__ f, float attn,
+                                  int64_t n_pos, const int64_t* __restrict__ st) {
+  const int j = blockIdx.y, b = blockIdx.z;
+  const int64_t n = st != nullptr ? st[2 * b + 1] : n_pos;
+  const float fj = rotary_row_freq(theta, f != nullptr ? f + (int64_t)b * kHalf : nullptr, j);
+  const int64_t row = ((int64_t)b * kHalf + j) * n_pos;
+  for (int64_t pos64 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos64 < n; pos64 += (int64_t)gridDim.x * blockDim.x) {
+    const float2 cs = rope_cos_sin(fj, (int)pos64);
     const float2 e = make_float2(cs.x * attn, cs.y * attn);
     if constexpr (HALF) {
       const __half2 h = __floats2half2_rn(e.x, e.y);
-      static_cast<uint32_t*>(out)[(int64_t)j * n_pos + pos64] = *reinterpret_cast<const uint32_t*>(&h);
+      static_cast<uint32_t*>(out)[row + pos64] = *reinterpret_cast<const uint32_t*>(&h);
     } else {
-      static_cast<float2*>(out)[(int64_t)j * n_pos + pos64] = e;
+      static_cast<float2*>(out)[row + pos64] = e;
     }
   }
+}
+
+// the static tables of kvq_rope_table_build*: one shared table, every argument checked before anything is launched
+static int rope_table_build(void* out, float theta, const float* freq, float attn, int64_t n_pos, void* stream,
+                            bool half) {
+  const dim3 grid((unsigned)((n_pos + 255) / 256 > 4096 ? 4096 : (n_pos + 255) / 256), kHalf);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (half) rope_table_kernel<true><<<grid, 256, 0, st>>>(out, theta, freq, attn, n_pos, nullptr);
+  else rope_table_kernel<false><<<grid, 256, 0, st>>>(out, theta, freq, attn, n_pos, nullptr);
+  KVQ_LAUNCH_CHECK();
+  return 0;
 }
 
 // Length-dependent rotary frequencies (kvq_rope_len_update, DESIGN.md section 4.14).  Per sequence b: f_cur [b][64],
@@ -596,22 +558,6 @@ __global__ void rope_len_prepare_kernel(int mode, double theta, double factor, i
     const bool rebuild = sb[0] != key;
     sb[0] = key;
     sb[1] = rebuild ? (end < npos ? end : npos) : 0;
-  }
-}
-
-// positions [0, st[b][1]) of sequence b's table from f_cur[b] -- rope_table_freq_kernel<false>'s expressions, bit for
-// bit its entries; st[b][1] == 0 exits at once.  grid = (x, 64, B).
-__global__ void rope_len_rebuild_kernel(const float* __restrict__ f_cur, const int64_t* __restrict__ st, float attn,
-                                        float2* __restrict__ table, int64_t npos) {
-  const int j = blockIdx.y, b = blockIdx.z;
-  const int64_t n = st[2 * b + 1];
-  const int64_t p0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p0 >= n) return;
-  const float f = f_cur[(int64_t)b * kHalf + j];
-  float2* row = table + ((int64_t)b * kHalf + j) * npos;
-  for (int64_t pos64 = p0; pos64 < n; pos64 += (int64_t)gridDim.x * blockDim.x) {
-    const float2 cs = rope_cos_sin(f, (int)pos64);
-    row[pos64] = make_float2(cs.x * attn, cs.y * attn);
   }
 }
 
@@ -700,27 +646,18 @@ int k_scores_batch(const AttendCall& c, const AttendScratch& s) {
     k_batch_zero_kernel<<<dim3((unsigned)std::min<int64_t>((c.L + 2047) / 2048, 64), H, B), 256, 0, c.stream>>>(
         s.scores, s.stride, s.bstride, c.len_dev, c.len_add, c.L);
     KVQ_LAUNCH_CHECK();
-    const int rc = set_k_outlier_smem(smem + kOutThetaBytes, grp > 1, true, c.pg != nullptr, c.freq, c.rope_per_seq);
+    const int rc = set_k_outlier_smem(smem + kOutThetaBytes, grp > 1, true, c.pg != nullptr);
     if (rc != 0) return rc;
     const dim3 grid(k_outlier_grid(c.L * c.n_out, smem, B), (unsigned)B);
     const bool direct = k_out_direct(c.L + c.pos_offset, false);
-    const float direct_theta = direct ? c.theta : 0.f;
     const int64_t b_rows = c.pg != nullptr ? 0 : c.Lmax * c.n_out;   // a pool has no per-sequence row block
     const float2* rope = reinterpret_cast<const float2*>(c.rope);
     const PageRef pg = c.pg != nullptr ? *c.pg : PageRef{};
     with_flavour(grp > 1, true, c.pg != nullptr, [&](auto GQA, auto BATCH, auto PAGED) {
-      if (c.rope_per_seq)
-        k_outlier_pers_seq_kernel<GQA(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
-            c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, rope, c.rope_npos, c.pos_offset,
-            1.f, c.len_dev, c.len_add, direct ? c.rope_freq : nullptr, c.attn_factor, grp, s.bstride, b_rows, pg);
-      else if (c.freq)
-        k_outlier_pers_freq_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
-            c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, rope, c.rope_npos, c.pos_offset,
-            1.f, c.len_dev, c.len_add, nullptr, direct ? c.rope_freq : nullptr, c.attn_factor, grp, s.bstride, b_rows, pg);
-      else
-        k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
-            c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, rope, c.rope_npos, c.pos_offset,
-            1.f, c.len_dev, c.len_add, nullptr, direct_theta, grp, s.bstride, b_rows, pg);
+      k_outlier_pers_kernel<GQA(), BATCH(), PAGED()><<<grid, kOutPersThreads, smem + kOutThetaBytes, c.stream>>>(
+          c.q, c.k_outliers, c.k_outlier_idx, s.scores, s.stride, 1, c.L, H, c.n_out, rope, c.rope_npos, c.pos_offset,
+          1.f, c.len_dev, c.len_add, nullptr, c.theta, c.freq ? c.rope_freq : nullptr, c.freq ? c.attn_factor : 1.f,
+          direct, grp, s.bstride, b_rows, pg, c.rope_per_seq ? kHalf * c.rope_npos : 0, c.rope_per_seq ? kHalf : 0);
     });
     KVQ_LAUNCH_CHECK();
     accumulate = 1;
@@ -737,21 +674,20 @@ extern "C" {
 int kvq_rope_table_build(float* rope_cos_sin, float theta, int64_t n_pos, void* stream) {
   if (!rope_cos_sin) return KVQ_E_NULL;
   if (n_pos <= 0 || n_pos > (int64_t)1 << 30) return KVQ_E_SHAPE;
-  const dim3 grid((unsigned)((n_pos + 255) / 256 > 4096 ? 4096 : (n_pos + 255) / 256), kHalf);
-  rope_table_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(reinterpret_cast<float2*>(rope_cos_sin), theta, n_pos);
-  KVQ_LAUNCH_CHECK();
-  return 0;
+  return rope_table_build(rope_cos_sin, theta, nullptr, 1.f, n_pos, stream, false);
 }
 
-// scaled tables: every argument is checked before anything is launched, the frequency vector is read on the device
+int kvq_rope_table_build_half(void* rope_half, float theta, int64_t n_pos, void* stream) {
+  if (!rope_half) return KVQ_E_NULL;
+  if (n_pos <= 0 || n_pos > (int64_t)1 << 30) return KVQ_E_SHAPE;
+  return rope_table_build(rope_half, theta, nullptr, 1.f, n_pos, stream, true);
+}
+
+// scaled tables: the frequency vector is read on the device
 static int rope_table_freq_build(void* out, const float* freq, float attn_factor, int64_t n_pos, void* stream, bool half) {
   if (!out || !freq) return KVQ_E_NULL;
   if (n_pos <= 0 || n_pos > (int64_t)1 << 30 || !(attn_factor > 0.f && attn_factor < INFINITY)) return KVQ_E_SHAPE;
-  const dim3 grid((unsigned)((n_pos + 255) / 256 > 4096 ? 4096 : (n_pos + 255) / 256), kHalf);
-  if (half) rope_table_freq_kernel<true><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(out, freq, attn_factor, n_pos);
-  else rope_table_freq_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(out, freq, attn_factor, n_pos);
-  KVQ_LAUNCH_CHECK();
-  return 0;
+  return rope_table_build(out, 0.f, freq, attn_factor, n_pos, stream, half);
 }
 
 int kvq_rope_table_build_freq(float* rope_cos_sin, const float* freq, float attn_factor, int64_t n_pos, void* stream) {
@@ -778,7 +714,7 @@ int kvq_rope_len_update(int mode, const double* params, int64_t m_pos, const flo
   KVQ_LAUNCH_CHECK();
   // a second launch: no rebuild CTA reads a sequence's decision while the prepare CTA writes it
   const dim3 grid((unsigned)((npos + 255) / 256 > 16 ? 16 : (npos + 255) / 256), kHalf, (unsigned)B);
-  rope_len_rebuild_kernel<<<grid, 256, 0, st>>>(f_cur, state, attn_factor, reinterpret_cast<float2*>(table), npos);
+  rope_table_kernel<false><<<grid, 256, 0, st>>>(table, 0.f, f_cur, attn_factor, npos, state);
   KVQ_LAUNCH_CHECK();
   return 0;
 }

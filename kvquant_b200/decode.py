@@ -237,7 +237,6 @@ class DecoderStage:
         lib = _lib.load()
         b = self._buffers()
         H, hid = cfg.n_heads, cfg.hidden
-        gqa = cfg.kv_heads != H
         st = torch.cuda.current_stream().cuda_stream
         xs = (b["x0"], b["x1"])     # ping-pong residual stream (the caller's x is never written)
         flip = 0
@@ -250,28 +249,19 @@ class DecoderStage:
             else:
                 rot = self.rope_state.update(s=c0.n_sink + c0.pos_base + c0.len + 1)
             freq = rot.f_cur
+        attn = self.rotary.attention_factor if self.rotary is not None else 1.0   # theta: 1, an exact product
         for ly in self.layers:
             c = ly.cache
             dyn = self.dyn          # device-resident length / position (one graph for a growing cache) or None
             self._gemv(ly.wqkv, x, 3, b["qkv"], norm_w=ly.n1)
-            if self.rotary is not None:   # (unsharded): position *pos_dev, or the host position
-                pos = (dyn["pos"].data_ptr(), 0) if dyn is not None else (None, c.n_sink + c.pos_base + c.len)
-                _lib.check(lib.kvq_dec_rope_split_freq(b["qkv"].data_ptr(), freq.data_ptr(),
-                                                       self.rotary.attention_factor, *pos, b["q"].data_ptr(),
-                                                       b["k"].data_ptr(), b["v"].data_ptr(), H, cfg.kv_heads, 1, st),
-                           "kvq_dec_rope_split_freq")
-            elif dyn is None:
-                # absolute position of the new token
-                pos = self.global_pos if self.sp is not None else c.n_sink + c.pos_base + c.len
-                qkv = (b["qkv"].data_ptr(), self.inv_freq.data_ptr(), float(pos),
-                       b["q"].data_ptr(), b["k"].data_ptr(), b["v"].data_ptr())
-                _lib.check(lib.kvq_dec_rope_split_gqa(*qkv, H, cfg.kv_heads, st) if gqa
-                           else lib.kvq_dec_rope_split(*qkv, hid, st))
+            # the new token's absolute position: *pos_dev, or the host position
+            if dyn is not None:
+                pos = (dyn["pos"].data_ptr(), 0)
             else:
-                qkv = (b["qkv"].data_ptr(), self.inv_freq.data_ptr(), dyn["pos"].data_ptr(), 0,
-                       b["q"].data_ptr(), b["k"].data_ptr(), b["v"].data_ptr())
-                _lib.check(lib.kvq_dec_rope_split_gqa_dyn(*qkv, H, cfg.kv_heads, st) if gqa
-                           else lib.kvq_dec_rope_split_dyn(*qkv, hid, st))
+                pos = (None, self.global_pos if self.sp is not None else c.n_sink + c.pos_base + c.len)
+            _lib.check(lib.kvq_dec_rope_split_freq(b["qkv"].data_ptr(), freq.data_ptr(), attn, *pos, b["q"].data_ptr(),
+                                                   b["k"].data_ptr(), b["v"].data_ptr(), H, cfg.kv_heads, 1, st),
+                       "kvq_dec_rope_split_freq")
             qh = b["q"].view(H, HEAD_DIM)
             if self.sp is None:
                 if dyn is None:
@@ -524,7 +514,7 @@ class BatchedDecoderStage:
 
     Each layer gets a BatchedLayerCache (the stage's calibration and sinks, one per slot) and every layer shares one
     device length tensor `lens` [B].  A step reads x fp16 [B, hidden]: RMSNorm + the fused QKV projection as one fp16
-    matmul, kvq_dec_rope_split_batch (row b at position n_sink + lens[b]), the batched append and attend, o_proj +
+    matmul, kvq_dec_rope_split_freq (row b at position n_sink + lens[b]), the batched append and attend, o_proj +
     residual and the MLP with the math of DecoderStage.forward_torch / prefill (torch matmuls), then lens += 1 for the
     active slots -- nothing touches the host, so the step can be captured (BatchedGraphedStep).  A slot is filled with
     prefill_seq(b, x) through its sequence views, and retired with reset_seq(b).  The attend of a slot that is not
@@ -654,20 +644,14 @@ class BatchedDecoderStage:
             rot = self.rope_state.update(len_dev=self.lens, len_add=1, L_cap=bc0.Lmax, pos_offset=bc0.n_sink)
         for ly, bc in zip(self.stage.layers, self.caches):
             qkv = (rmsnorm(x, ly.n1, cfg.rms_eps) @ ly.wqkv.t()).contiguous()
-            if isinstance(rot, RopeLenState):
-                _lib.check(lib.kvq_dec_rope_split_freq_seq(
-                    qkv.data_ptr(), rot.f_cur.data_ptr(), rot.spec.attention_factor, self.lens.data_ptr(),
-                    bc.n_sink, self._q.data_ptr(), self._k.data_ptr(), self._v.data_ptr(), cfg.n_heads, cfg.kv_heads, B,
-                    st), "kvq_dec_rope_split_freq_seq")
-            elif rot is None:
-                _lib.check(lib.kvq_dec_rope_split_batch(
-                    qkv.data_ptr(), self.stage.inv_freq.data_ptr(), self.lens.data_ptr(), bc.n_sink, self._q.data_ptr(),
-                    self._k.data_ptr(), self._v.data_ptr(), cfg.n_heads, cfg.kv_heads, B, st), "kvq_dec_rope_split_batch")
+            if isinstance(rot, RopeLenState):   # row b at its own frequencies
+                fn, freq, attn = "kvq_dec_rope_split_freq_seq", rot.f_cur, rot.spec.attention_factor
             else:
-                _lib.check(lib.kvq_dec_rope_split_freq(
-                    qkv.data_ptr(), self.stage.inv_freq.data_ptr(), rot.attention_factor, self.lens.data_ptr(),
-                    bc.n_sink, self._q.data_ptr(), self._k.data_ptr(), self._v.data_ptr(), cfg.n_heads, cfg.kv_heads, B,
-                    st), "kvq_dec_rope_split_freq")
+                fn, freq = "kvq_dec_rope_split_freq", self.stage.inv_freq
+                attn = rot.attention_factor if rot is not None else 1.0
+            _lib.check(getattr(lib, fn)(qkv.data_ptr(), freq.data_ptr(), attn, self.lens.data_ptr(), bc.n_sink,
+                                        self._q.data_ptr(), self._k.data_ptr(), self._v.data_ptr(), cfg.n_heads,
+                                        cfg.kv_heads, B, st), fn)
             bc.append_dyn(self._k, self._v, active=self.active)
             o = bc.attend(self._q, out=self._o, len_add=1, rope_theta=cfg.rope_theta, rope=rot)
             x = x + o.half().view(B, hid) @ ly.wo.t()

@@ -13,7 +13,7 @@ and B = 256, and records the geometry it reached in its assertion messages.
   bit for bit on dense caches, within 8 fp32 ulps of each head's max with outlier rows -- and against float64 at 256;
 * batched and paged appends at B = 67 and 256 against single caches (inactive and full slots, page crossings);
 * one contiguous batch whose K / V slices start past 2^31 words;
-* LLaMA-3.1 scaled rotary (k_outlier_pers_freq_kernel with one K range per sequence) against float64;
+* LLaMA-3.1 scaled rotary (k_outlier_pers_kernel with a frequency vector, one K range per sequence) against float64;
 * a 2-layer LLaMA-3-8B BatchedDecoderStage graph at B = 67, contiguous and paged, against single-sequence runs;
 * kvq_dec_rope_split_batch / _freq at B = 256 and at the grid-y limit 65535 against HF's rotation in float64.
 The geometry helper is checked against hand-derived thresholds without a GPU.
@@ -370,8 +370,8 @@ def test_sequence_slices_past_2_31_words():
 @gpu
 @pytest.mark.parametrize("paged", (False, True))
 def test_llama31_rotary_at_scale(paged):
-    """LLaMA-3.1 rotary at B = 67, 3 bits, 32/8, K+V outliers: the batched (and paged) k_outlier_pers_freq_kernel
-    with one K range per sequence on a 132-SM H100, against float64 from HF's fp32 angles."""
+    """LLaMA-3.1 rotary at B = 67, 3 bits, 32/8, K+V outliers: the batched (and paged) k_outlier_pers_kernel with a
+    frequency vector, one K range per sequence on a 132-SM H100, against float64 from HF's fp32 angles."""
     spec = R.LLAMA31
     bits, Hq, Hkv, B, Lmax = 3, 32, 8, 67, 1120
     geo = _geometry(bits, Hq, Hkv, B)
