@@ -208,7 +208,8 @@ KVQ_API int kvq_attend_dyn(int bits, const float* q, const int32_t* kcache, cons
  * head h / g (HF repeat_kv, scaled_dot_product_attention(enable_gqa=True)).  The cache is an ordinary Hkv-head cache:
  * append, dequantisation, outlier rows (channels index the Hkv*128 KV hidden) and tables are those of H = Hkv.  Sinks
  * belong to the cache: sink_k f16 [Hkv,128,n_sink], sink_v f16 [Hkv,n_sink,128].  q, out f32 [Hq,128], out_lse [Hq].
- *   Shapes: Hq <= 64, Hq % 4 == 0, Hkv % 4 == 0, Hq % Hkv == 0; anything else is KVQ_E_SHAPE.
+ *   Shapes: Hq <= 64, Hq % 4 == 0, Hq % Hkv == 0, and Hkv % 4 == 0 or Hkv in {1, 2} (two-KV-head and multi-query
+ *   models); anything else is KVQ_E_SHAPE.
  *   kvq_attend_gqa / kvq_attend_gqa_dyn: kvq_attend / kvq_attend_dyn with (Hq, Hkv) in place of H; scratch of
  *   kvq_attend_scratch_bytes(Hq, L) (or L_cap) bytes.  With Hq == Hkv they are kvq_attend / kvq_attend_dyn.  With
  *   g > 1: native V form (v_cent + v_aff) and exact tables only -- a missing v_cent / v_aff or a non-NULL rope_half
@@ -269,7 +270,7 @@ KVQ_API int kvq_attend_gqa_dyn_freq(int bits, const float* q, const int32_t* kca
  * len_dev int64 [B] (device).  The K LUTs, thresholds and centroids are shared (one layer's calibration).
  *   kvq_append_kv_fused_batch: k_new, v_new f32 [B, Hkv*128]; sequence b writes slot len_dev[b] + slot_add, bit for bit
  *     what kvq_append_kv_fused_dyn writes into a single cache; a full sequence drops its token; active (int32 [B], or
- *     NULL = all) == 0 writes nothing.  One launch, grid (2, B).  1 <= B <= 256, Hkv % 4 == 0.
+ *     NULL = all) == 0 writes nothing.  One launch, grid (2, B).  1 <= B <= 256, Hkv % 4 == 0 or Hkv <= 2.
  *   kvq_attend_batch: q f32 [B, Hq, 128]; sequence b attends over min(len_dev[b] + len_add, L_cap) slots plus its own
  *     n_sink sinks, slot t at position pos_offset + t; out f32 [B, Hq, 128], out_lse f32 [B, Hq] or NULL.  There is
  *     no active mask: with len_add > 0 a sequence that did not append this step attends a slot it never wrote, and
@@ -442,6 +443,7 @@ KVQ_API int kvq_append_kv_fused_chunk(int bits, int H, int64_t Lmax, int64_t slo
  *   V: value = v_cent[code]*sf_t + off_t (one fma; v_cent = the Q-Norm-shifted centroids when V Q-Norm is on, (sf_t,
  *      off_t) = v_aff row t) + the V outlier residual.  Native V form only (like kvq_attend_dyn).
  *   k_outliers / v_outliers pairs may be NULL (dense-only cache, or K outliers only); n_out <= 128, even.
+ *   H (the cache's KV heads) <= 64 with H % 4 == 0 or H in {1, 2}; anything else is KVQ_E_SHAPE.
  *   start == stop returns 0 once the sizes are valid, whatever the pointers (an empty output may be NULL), and
  *   launches nothing.  All offsets are 64-bit.  Two launches (K, V) on `stream`.
  * ------------------------------------------------------------------------------------------------------------- */

@@ -155,9 +155,11 @@ class LayerCache:
         if self.Lmax % 4:
             raise ValueError("max_len must be a multiple of 4 (TMA row pitch)")
         self.Hq = self.H if q_heads is None else int(q_heads)
-        if self.Hq != self.H and (self.H <= 0 or self.H % 4 or self.Hq % 4 or self.Hq > 64 or self.Hq % self.H):
-            raise ValueError("grouped-query attention needs q_heads <= 64, q_heads %% 4 == 0, KV heads %% 4 == 0 and "
-                             "q_heads a multiple of the KV heads; got q_heads=%d, KV heads=%d" % (self.Hq, self.H))
+        if self.Hq != self.H and (self.H <= 0 or (self.H % 4 and self.H > 2) or self.Hq % 4 or self.Hq > 64
+                                  or self.Hq % self.H):
+            raise ValueError("grouped-query attention needs q_heads <= 64, q_heads %% 4 == 0, KV heads %% 4 == 0 or "
+                             "KV heads in {1, 2}, and q_heads a multiple of the KV heads; got q_heads=%d, KV heads=%d"
+                             % (self.Hq, self.H))
         self.group = self.Hq // self.H       # query heads per KV head (1: one KV head per query head)
         self.hidden = self.H * HEAD_DIM
         self.q_hidden = self.Hq * HEAD_DIM

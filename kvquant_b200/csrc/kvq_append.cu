@@ -840,7 +840,8 @@ static int append_kv_fused_impl(int bits, int H, int64_t Lmax, int64_t slot, con
     return KVQ_E_NULL;
   const int hidden = H * kHeadDim;
   if (H <= 0 || hidden > kMaxHidden || Lmax <= 0) return KVQ_E_SHAPE;
-  if (B > 0 && (H % 4 != 0 || Lmax % 4 != 0)) return KVQ_E_SHAPE;   // the batch strides keep every slice 16-byte aligned
+  // the batch strides keep every slice 16-byte aligned (Lmax % 4 == 0); H as the attends accept it: H % 4 == 0 or H <= 2
+  if (B > 0 && ((H % 4 != 0 && H > 2) || Lmax % 4 != 0)) return KVQ_E_SHAPE;
   if (slot_dev == nullptr && (slot < 0 || slot >= Lmax)) return KVQ_E_SHAPE;
   const bool any_sparse = k_outliers != nullptr || v_outliers != nullptr;
   if (any_sparse && (n_each <= 0 || 2 * n_each > kMaxOut || 2 * (n_each + 1) > hidden)) return KVQ_E_SHAPE;

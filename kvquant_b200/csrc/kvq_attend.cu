@@ -146,8 +146,9 @@ AttendScratch attend_scratch(void* scratch, int H, int64_t L, int bits) {
 
 // Grouped-query attention: Hq query heads over an Hkv-head cache, query head h attending over KV head h / (Hq / Hkv).
 // Hq == Hkv is multi-head attention, every K and V form; otherwise the exact-table, native-V path only.
+// Hq % 4 == 0, Hq <= 64, and Hkv % 4 == 0 or Hkv <= 2 (two-KV-head and multi-query models, DESIGN.md section 4.9).
 static int check_gqa(int Hq, int Hkv) {
-  if (Hkv <= 0 || Hq <= 0 || Hq > 64 || (Hq & 3) != 0 || (Hkv & 3) != 0 || Hq % Hkv != 0) return KVQ_E_SHAPE;
+  if (Hkv <= 0 || Hq <= 0 || Hq > 64 || (Hq & 3) != 0 || ((Hkv & 3) != 0 && Hkv > 2) || Hq % Hkv != 0) return KVQ_E_SHAPE;
   return 0;
 }
 static int gqa_unsupported(const AttendCall& c) {

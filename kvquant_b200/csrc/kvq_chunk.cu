@@ -438,7 +438,7 @@ static int attend_chunk_impl(int bits, int H, int Hkv, int64_t Lmax, int64_t L, 
                              void* scratch, void* stream) {
   if (bits < 2 || bits > 4) return KVQ_E_BITS;
   if (H <= 0 || (H & 3) != 0 || H > 64 || Lmax <= 0 || L < 0 || L > Lmax || T < 0) return KVQ_E_SHAPE;
-  if (Hkv <= 0 || (Hkv & 3) != 0 || H % Hkv != 0) return KVQ_E_SHAPE;
+  if (Hkv <= 0 || ((Hkv & 3) != 0 && Hkv > 2) || H % Hkv != 0) return KVQ_E_SHAPE;
   if (n_out < 0 || (n_out & 1) != 0 || n_out > kMaxOutDq) return KVQ_E_SHAPE;
   if (n_sink < 0 || pos_offset < 0 || rope_npos < (int64_t)pos_offset + L) return KVQ_E_SHAPE;
   if (T == 0) return 0;   // nothing to attend: no launch

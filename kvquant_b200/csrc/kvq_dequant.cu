@@ -21,7 +21,7 @@
 namespace kvq {
 
 constexpr int kTile = 32;       // tokens per tile
-constexpr int kGroup = 2;       // heads per CTA (every accepted H is a multiple of 4)
+constexpr int kGroup = 2;       // heads per CTA (every accepted H but 1 is even; H = 1: dequant_one_kernel)
 constexpr int kThreads = 256;
 constexpr int kRopePitch = 65;  // float2 per staged cos/sin row (one token); odd pitch spreads the transposing writes
 constexpr int kTP = kHeadDim + 4;  // fp32 tile row pitch (one token of one head)
@@ -42,21 +42,21 @@ struct DqParams {
   int n_out;
 };
 
-template <int BITS>
+template <int BITS, int NG = kGroup>   // NG: heads per CTA
 struct DqLayout {
   static constexpr int W = Layout<BITS>::kWords;
   static constexpr int kWPitch = W + 1;  // odd pitch: the transposing word stores of a warp hit distinct banks
-  static constexpr int kWordsSmem = kGroup * kTile * kWPitch;
-  static constexpr int kTileSmem = kGroup * kTile * kTP;
+  static constexpr int kWordsSmem = NG * kTile * kWPitch;
+  static constexpr int kTileSmem = NG * kTile * kTP;
   static constexpr int kLP = Layout<BITS>::kLevels + 1;   // K LUT pitch per channel
 };
 
-template <int BITS>
+template <int BITS, int NG = kGroup>
 __host__ __device__ constexpr size_t dq_smem_bytes(bool is_v, bool rope) {
-  using D = DqLayout<BITS>;
+  using D = DqLayout<BITS, NG>;
   return sizeof(float) * (D::kTileSmem + D::kWordsSmem) +
          (is_v ? sizeof(float) * (Layout<BITS>::kLevels + 2 * kTile)
-               : sizeof(float) * DqLayout<BITS>::kLP * kGroup * kHeadDim + (rope ? sizeof(float2) * kTile * kRopePitch : 0));
+               : sizeof(float) * D::kLP * NG * kHeadDim + (rope ? sizeof(float2) * kTile * kRopePitch : 0));
 }
 
 // IS_V: V side (affine centroids) else K side (per-channel LUT, optional rotation).
@@ -64,24 +64,24 @@ __host__ __device__ constexpr size_t dq_smem_bytes(bool is_v, bool rope) {
 // [n_pool*P, .]) and pg.table is one sequence's page-table row; slot s is read from page pg.table[s / P], column s % P.
 // The tiles are the contiguous kernel's, and every read looks its token's page up (a 32-token tile starting at any
 // `start` may straddle a page boundary); the arithmetic and the output offsets are those of logical slots.
-template <int BITS, bool IS_V, bool ROPE, bool PAGED>
+template <int BITS, bool IS_V, bool ROPE, bool PAGED, int NG = kGroup>
 __device__ __forceinline__ void dequant_body(const DqParams& p, const PageRef& pg) {
-  using D = DqLayout<BITS>;
+  using D = DqLayout<BITS, NG>;
   constexpr int W = D::W;
   constexpr int NL = Layout<BITS>::kLevels;
   extern __shared__ __align__(16) float smem[];
-  float* tile = smem;                                                       // [kGroup][kTile][kTP]
-  uint32_t* words = reinterpret_cast<uint32_t*>(tile + D::kTileSmem);       // [kGroup][kTile][kWPitch]
-  float* tab = reinterpret_cast<float*>(words + D::kWordsSmem);             // K: LUT [kGroup*128][kLP]; V: cent[NL], aff[kTile][2]
-  float2* cs = reinterpret_cast<float2*>(tab + D::kLP * kGroup * kHeadDim); // K + ROPE: [kTile][kRopePitch]
+  float* tile = smem;                                                       // [NG][kTile][kTP]
+  uint32_t* words = reinterpret_cast<uint32_t*>(tile + D::kTileSmem);       // [NG][kTile][kWPitch]
+  float* tab = reinterpret_cast<float*>(words + D::kWordsSmem);             // K: LUT [NG*128][kLP]; V: cent[NL], aff[kTile][2]
+  float2* cs = reinterpret_cast<float2*>(tab + D::kLP * NG * kHeadDim); // K + ROPE: [kTile][kRopePitch]
   float* aff = tab + NL;
 
   const int tid = threadIdx.x;
-  const int h0 = blockIdx.y * kGroup;
+  const int h0 = blockIdx.y * NG;
   if constexpr (IS_V) {
     if (tid < NL) tab[tid] = p.v_cent[tid];
   } else {
-    for (int i = tid; i < kGroup * kHeadDim * NL; i += kThreads)
+    for (int i = tid; i < NG * kHeadDim * NL; i += kThreads)
       tab[(i / NL) * D::kLP + i % NL] = p.klut[(int64_t)h0 * kHeadDim * NL + i];
   }
 
@@ -97,16 +97,16 @@ __device__ __forceinline__ void dequant_body(const DqParams& p, const PageRef& p
       int64_t base = 0;                                       // word row 0 of the group at token t's page column
       if (t < nt) {
         const PageCol pc = page_col(pg, (int)(t0 + t));
-        base = ((int64_t)pc.page * gridDim.y * kGroup + h0) * W * pg.P + pc.col;
+        base = ((int64_t)pc.page * gridDim.y * NG + h0) * W * pg.P + pc.col;
       }
-      for (int i = tid; i < kGroup * W * kTile; i += kThreads) {
+      for (int i = tid; i < NG * W * kTile; i += kThreads) {
         const int r = i / kTile;
         uint32_t w = 0;
         if (t < nt) w = static_cast<uint32_t>(p.cache[base + (int64_t)r * pg.P]);
         words[((r / W) * kTile + t) * D::kWPitch + (r % W)] = w;
       }
     } else {
-      for (int i = tid; i < kGroup * W * kTile; i += kThreads) {
+      for (int i = tid; i < NG * W * kTile; i += kThreads) {
         const int r = i / kTile, t = i % kTile;               // r: word row within the group, t fastest (coalesced)
         uint32_t w = 0;
         if (t < nt) w = static_cast<uint32_t>(p.cache[((int64_t)h0 * W + r) * p.Lmax + t0 + t]);
@@ -126,7 +126,7 @@ __device__ __forceinline__ void dequant_body(const DqParams& p, const PageRef& p
       }
     }
     __syncthreads();
-    for (int i = tid; i < kGroup * kTile * 4; i += kThreads) {
+    for (int i = tid; i < NG * kTile * 4; i += kThreads) {
       const int t = i % kTile, q = (i / kTile) % 4, g = i / (4 * kTile);   // lanes: 32 tokens of one channel group
       constexpr int WQ = W / 4;                                // words of 32 channels: 4 / 3 / 2
       uint32_t w[WQ];
@@ -144,14 +144,14 @@ __device__ __forceinline__ void dequant_body(const DqParams& p, const PageRef& p
           const int64_t e = page_row(pg, (int)(t0 + j)) * p.n_out + (i - j * p.n_out);
           const int idx = p.outlier_idx[e];
           const int g = (idx >> 7) - h0;
-          if (g >= 0 && g < kGroup) dq_add_outlier(&tile[(g * kTile + j) * kTP + (idx & 127)], p.outliers[e]);
+          if (g >= 0 && g < NG) dq_add_outlier(&tile[(g * kTile + j) * kTP + (idx & 127)], p.outliers[e]);
         }
       } else {
         const int64_t row0 = t0 * p.n_out;
         for (int i = tid; i < nt * p.n_out; i += kThreads) {
           const int idx = p.outlier_idx[row0 + i];
           const int g = (idx >> 7) - h0;
-          if (g >= 0 && g < kGroup) {
+          if (g >= 0 && g < NG) {
             const float v = p.outliers[row0 + i];
             dq_add_outlier(&tile[(g * kTile + i / p.n_out) * kTP + (idx & 127)], v);
           }
@@ -159,7 +159,7 @@ __device__ __forceinline__ void dequant_body(const DqParams& p, const PageRef& p
       }
     }
     __syncthreads();
-    for (int i = tid; i < kGroup * kTile * (kHeadDim / 8); i += kThreads) {
+    for (int i = tid; i < NG * kTile * (kHeadDim / 8); i += kThreads) {
       const int q = i % (kHeadDim / 8), gt = i / (kHeadDim / 8);
       const int t = gt % kTile, g = gt / kTile;
       if (t >= nt) continue;
@@ -185,13 +185,23 @@ __global__ void __launch_bounds__(kThreads, 3) dequant_paged_kernel(const DqPara
   dequant_body<BITS, IS_V, ROPE, true>(p, pg);
 }
 
+// one KV head (H = 1, multi-query caches): CTAs of one head, contiguous (pg.table == nullptr) or paged.  Kernels of
+// their own name: an NG template argument would rename the instantiations above.
+template <int BITS, bool IS_V, bool ROPE>
+__global__ void __launch_bounds__(kThreads, 3) dequant_one_kernel(const DqParams p, const PageRef pg) {
+  if (pg.table == nullptr) dequant_body<BITS, IS_V, ROPE, false, 1>(p, pg);
+  else dequant_body<BITS, IS_V, ROPE, true, 1>(p, pg);
+}
+
 template <int BITS, bool IS_V, bool ROPE>
 int launch_dequant(const DqParams& p, int H, cudaStream_t st, const PageRef* pg) {
-  const void* kern = pg != nullptr ? reinterpret_cast<const void*>(dequant_paged_kernel<BITS, IS_V, ROPE>)
-                                   : reinterpret_cast<const void*>(dequant_kernel<BITS, IS_V, ROPE>);
-  const size_t smem = dq_smem_bytes<BITS>(IS_V, ROPE);
-  static PerDeviceOnce attr_once[2];   // (per form)
-  bool& attr_done = attr_once[pg != nullptr].cur();
+  const bool one = H == 1;
+  const void* kern = one ? reinterpret_cast<const void*>(dequant_one_kernel<BITS, IS_V, ROPE>)
+                     : pg != nullptr ? reinterpret_cast<const void*>(dequant_paged_kernel<BITS, IS_V, ROPE>)
+                                     : reinterpret_cast<const void*>(dequant_kernel<BITS, IS_V, ROPE>);
+  const size_t smem = one ? dq_smem_bytes<BITS, 1>(IS_V, ROPE) : dq_smem_bytes<BITS>(IS_V, ROPE);
+  static PerDeviceOnce attr_once[3];   // (per form)
+  bool& attr_done = attr_once[one ? 2 : pg != nullptr].cur();
   if (!attr_done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
@@ -204,11 +214,12 @@ int launch_dequant(const DqParams& p, int H, cudaStream_t st, const PageRef* pg)
   if (e != cudaSuccess) return (int)e;
   // one wave of resident CTAs: the head groups side by side (they read the same tile's outlier rows and cos/sin at
   // about the same time), the token tiles split evenly over the rest
-  const int groups = H / kGroup;
+  const int groups = one ? 1 : H / kGroup;
   const int64_t n_tiles = (p.stop - p.start + kTile - 1) / kTile;
   const int64_t per_group = max(1, sms * max(per_sm, 1) / groups);
   const dim3 grid((unsigned)min(n_tiles, per_group), (unsigned)groups);
-  if (pg != nullptr) dequant_paged_kernel<BITS, IS_V, ROPE><<<grid, kThreads, smem, st>>>(p, *pg);
+  if (one) dequant_one_kernel<BITS, IS_V, ROPE><<<grid, kThreads, smem, st>>>(p, pg != nullptr ? *pg : PageRef{});
+  else if (pg != nullptr) dequant_paged_kernel<BITS, IS_V, ROPE><<<grid, kThreads, smem, st>>>(p, *pg);
   else dequant_kernel<BITS, IS_V, ROPE><<<grid, kThreads, smem, st>>>(p);
   KVQ_LAUNCH_CHECK();
   return 0;
@@ -231,7 +242,7 @@ static int dequant_impl(int bits, int H, int64_t Lmax, int64_t start, int64_t st
                         int n_out, const float* rope_cos_sin, int64_t rope_npos, int pos_offset, void* out_k,
                         void* out_v, int64_t head_stride, void* stream, const PageRef* pg) {
   if (bits < 2 || bits > 4) return KVQ_E_BITS;
-  if (H <= 0 || (H & 3) != 0 || H > 64 || Lmax < 0 || (Lmax == 0 && pg == nullptr) || start < 0 || start > stop ||
+  if (H <= 0 || ((H & 3) != 0 && H > 2) || H > 64 || Lmax < 0 || (Lmax == 0 && pg == nullptr) || start < 0 || start > stop ||
       stop > Lmax)
     return KVQ_E_SHAPE;
   if (n_out < 0 || (n_out & 1) != 0 || n_out > kMaxOutDq) return KVQ_E_SHAPE;

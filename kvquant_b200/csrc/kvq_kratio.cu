@@ -189,10 +189,14 @@ __device__ __forceinline__ float k_ratio_head(const uint32_t st, const uint32_t 
 // With BATCH, sequence b's rope table sits b * rope_bstride entries after sequence 0's: 64 * rope_npos for a rotation
 // per sequence (length-dependent frequencies, DESIGN.md section 4.14), 0 for one table shared by the batch.  It is the
 // last kernel argument, not a KRParams field, so that every other argument keeps its parameter-bank offset.
-template <int BITS, bool GQA, bool BATCH, bool PAGED = false>
-__global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_constant__ CUtensorMap tmap, const KRParams p,
-                                                                const int group, const int64_t bstride, const PageRef pg,
-                                                                const int64_t rope_bstride) {
+// SUB (with GQA; k_ratio_sub_kernel): a KV head has more query heads than one CTA's table holds (grp > GMAX, one or
+// two KV heads), so a CTA owns a sub-range of one KV head's query heads.  The grp heads of each KV head are cut into
+// nsub = ceil(grp / p.G) ranges of at most p.G heads, CTA row y being range y % nsub of KV head y / nsub; its producer
+// loads that KV head's slab once per round, and its first and last heads wait for and release the stage.  The nsub
+// CTAs of a KV head each read its slab (DESIGN.md section 4.9).
+template <int BITS, bool GQA, bool BATCH, bool PAGED, bool SUB>
+__device__ __forceinline__ void k_ratio_body(const CUtensorMap& tmap, const KRParams& p, const int group,
+                                             const int64_t bstride, const PageRef& pg, const int64_t rope_bstride) {
   using C = KRCfg<BITS>;
   constexpr int W = C::W;
   const int grp = GQA ? group : 1;
@@ -203,8 +207,9 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int S = p.n_stages;
-  const int h0 = blockIdx.y * p.G;
-  const int nh = min(p.G, p.H - h0);
+  const int nsub = SUB ? (grp + p.G - 1) / p.G : 1;
+  const int h0 = SUB ? (int)blockIdx.y / nsub * grp + (int)blockIdx.y % nsub * p.G : blockIdx.y * p.G;
+  const int nh = min(p.G, SUB ? ((int)blockIdx.y / nsub + 1) * grp - h0 : p.H - h0);
   const uint32_t tab_span = (uint32_t)p.G * C::kHeadTab;
   const uint32_t rat_span = (uint32_t)p.G * C::kHeadRat;
   unsigned char* s_tab = smem;                                         // [G][128][N] f32
@@ -259,7 +264,7 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
         const int nlive = min(kKRWarps, ncols - r * kKRWarps);
         const int nbox = (nlive + C::kBoxWarps - 1) / C::kBoxWarps;    // the last box may reach past the range: read-only
         const int x0 = (int)(t_begin + (int64_t)r * kKRWarps * kKRColTok);
-        for (int hl = 0; hl < (GQA ? nh / grp : nh); ++hl) {   // one slab per KV head
+        for (int hl = 0; hl < (SUB ? 1 : (GQA ? nh / grp : nh)); ++hl) {   // one slab per KV head
           if (wrapped) mbar_wait(&s_empty[s], ph);
           mbar_expect_tx(&s_full[s], (uint32_t)nbox * C::kBox);
           unsigned char* dst = s_stage + (size_t)s * C::kStage;
@@ -328,7 +333,7 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
       float* optr = p.out + boff + (int64_t)(h0 + hl) * p.out_stride + t;
       float old = 0.f;
       if (p.accumulate && live && mine && hs.half == 0) old = __ldcg(optr);
-      if (!GQA || hl % grp == 0) mbar_wait(&s_full[s], ph);
+      if (SUB ? hl == 0 : (!GQA || hl % grp == 0)) mbar_wait(&s_full[s], ph);
       if (live) {
         float acc = k_ratio_head<BITS>(stage0 + (uint32_t)s * C::kStage, tab0 + (uint32_t)hl * C::kHeadTab,
                                        rat0 + (uint32_t)hl * C::kHeadRat, hs, cs);
@@ -342,7 +347,7 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
           if (lane == 0) atomicMax(&s_max[hl], key);
         }
       }
-      if (!GQA || hl % grp == grp - 1) {
+      if (SUB ? hl == nh - 1 : (!GQA || hl % grp == grp - 1)) {
         __syncwarp();
         if (lane == 0) mbar_arrive(&s_empty[s]);
         if (++s == S) { s = 0; ph ^= 1u; }
@@ -357,6 +362,21 @@ __global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_con
       if (m > -INFINITY) atomic_max_float(p.gmax + boff + h0 + tid, m);
     }
   }
+}
+
+template <int BITS, bool GQA, bool BATCH, bool PAGED = false>
+__global__ void __launch_bounds__(kKRThreads, 1) k_ratio_kernel(const __grid_constant__ CUtensorMap tmap, const KRParams p,
+                                                                const int group, const int64_t bstride, const PageRef pg,
+                                                                const int64_t rope_bstride) {
+  k_ratio_body<BITS, GQA, BATCH, PAGED, false>(tmap, p, group, bstride, pg, rope_bstride);
+}
+
+// a kernel of its own name: a SUB template argument would rename the instantiations above
+template <int BITS, bool BATCH, bool PAGED>
+__global__ void __launch_bounds__(kKRThreads, 1) k_ratio_sub_kernel(const __grid_constant__ CUtensorMap tmap, const KRParams p,
+                                                                    const int group, const int64_t bstride, const PageRef pg,
+                                                                    const int64_t rope_bstride) {
+  k_ratio_body<BITS, true, BATCH, PAGED, true>(tmap, p, group, bstride, pg, rope_bstride);
 }
 
 // table T[h][c][code] = LUT * qe_c and ratios r_c = s_c q_{c^64} / qe_c (qe = q, or +-1e-30 where q is exactly 0);
@@ -387,13 +407,14 @@ __global__ void k_ratio_prep_kernel(const float* __restrict__ q, const float* __
   qrat[(int64_t)h * kHeadDim + gi * 16 + half * 8 + xy * 4 + k] = sg * qb / qa;
 }
 
-template <int BITS, bool GQA, bool BATCH, bool PAGED>
+template <int BITS, bool GQA, bool BATCH, bool PAGED, bool SUB>
 static int set_k_ratio_smem() {
   static PerDeviceOnce attr_once;
   bool& attr_done = attr_once.cur();
   if (!attr_done) {
-    const cudaError_t e = cudaFuncSetAttribute(k_ratio_kernel<BITS, GQA, BATCH, PAGED>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kKRSmemBudget);
+    const void* kern = SUB ? reinterpret_cast<const void*>(k_ratio_sub_kernel<BITS, BATCH, PAGED>)
+                           : reinterpret_cast<const void*>(k_ratio_kernel<BITS, GQA, BATCH, PAGED>);
+    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kKRSmemBudget);
     if (e != cudaSuccess) return (int)e;
     attr_done = true;
   }
@@ -413,10 +434,20 @@ static int launch_k_ratio(KRParams p, const AttendCall& c, const AttendScratch& 
         c.q, c.klut, s.qtab, s.qrat, grp, s.bstride);
   });
   KVQ_LAUNCH_CHECK();
-  // CTA head groups of at most GMAX query heads; under GQA whole KV-head groups (grp <= 16 <= GMAX)
-  const int Hkv = p.H / grp, kv_max = C::GMAX / grp;
-  const int groups = (Hkv + kv_max - 1) / kv_max;
-  p.G = (Hkv + groups - 1) / groups * grp;
+  // CTA head groups of at most GMAX query heads: whole KV-head groups while grp <= GMAX (every shape with Hkv % 4 == 0),
+  // else (one or two KV heads) nsub CTAs per KV head, each a sub-range of its query heads (k_ratio_sub_kernel)
+  const int Hkv = p.H / grp;
+  const bool sub = grp > C::GMAX;
+  int groups;
+  if (sub) {
+    const int nsub = (grp + C::GMAX - 1) / C::GMAX;
+    p.G = (grp + nsub - 1) / nsub;
+    groups = Hkv * nsub;
+  } else {
+    const int kv_max = C::GMAX / grp;
+    groups = (Hkv + kv_max - 1) / kv_max;
+    p.G = (Hkv + groups - 1) / groups * grp;
+  }
   const uint32_t tab_span = (uint32_t)p.G * (C::kHeadTab + C::kHeadRat);
   const uint32_t fixed = tab_span + 1024u /*align*/ + 8u * 20u + 4u * 64u + 64u;
   int S = (int)((kKRSmemBudget - fixed) / C::kStage);
@@ -425,7 +456,7 @@ static int launch_k_ratio(KRParams p, const AttendCall& c, const AttendScratch& 
   p.n_stages = S;
   const size_t smem = (size_t)tab_span + (size_t)S * C::kStage + 8u * (2 * S + 1) + 4u * p.G + 1024u;
   int rc = with_flavour(gqa, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
-    return set_k_ratio_smem<BITS, GQA(), BATCH(), PAGED()>();
+    return sub ? set_k_ratio_smem<BITS, GQA(), BATCH(), PAGED(), true>() : set_k_ratio_smem<BITS, GQA(), BATCH(), PAGED(), false>();
   });
   if (rc != 0) return rc;
   CUtensorMap tmap;
@@ -445,9 +476,12 @@ static int launch_k_ratio(KRParams p, const AttendCall& c, const AttendScratch& 
   const int64_t splits = (p.L + p.range - 1) / p.range;
   const dim3 grid = batch ? dim3((unsigned)splits, (unsigned)groups, (unsigned)B) : dim3((unsigned)splits, (unsigned)groups);
   const int64_t rope_bstride = c.rope_per_seq ? kHalf * p.rope_npos : 0;
+  const PageRef pg = paged ? *c.pg : PageRef{};
   with_flavour(gqa, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
-    k_ratio_kernel<BITS, GQA(), BATCH(), PAGED()><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, s.bstride,
-                                                                                  paged ? *c.pg : PageRef{}, rope_bstride);
+    if (sub)
+      k_ratio_sub_kernel<BITS, BATCH(), PAGED()><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, s.bstride, pg, rope_bstride);
+    else
+      k_ratio_kernel<BITS, GQA(), BATCH(), PAGED()><<<grid, kKRThreads, smem, st>>>(tmap, p, grp, s.bstride, pg, rope_bstride);
   });
   KVQ_LAUNCH_CHECK();
   return 0;

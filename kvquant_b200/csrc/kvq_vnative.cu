@@ -38,6 +38,7 @@ constexpr int kNTokPerWarp = kNT / (kNThreads / 32);   // outlier rows handled b
 // ~25-way one on the outlier weight gather.
 constexpr int kNWStride = 33;    // w      : scalar gathers, head h token t -> bank (h + t) % 32
 constexpr int kNWsStride = 36;   // w * sf : 16-byte reads, head h chunk q -> bank group (h + q) % 8
+constexpr int kVNPad3 = 3 + 8;    // v_native_kernel's padded-box 3-bit form (below)
 
 struct VNParams {
   const float* score;        // [H, score_stride] scaled scores
@@ -143,10 +144,17 @@ __device__ __forceinline__ void vn_tile_unit(const unsigned char* stage, uint32_
 // (sf, off) and outlier rows are pool rows.  A 32-token tile lies inside one page (P % 32 == 0), so each tile looks its
 // page up for the TMA row base, and token t's (sf, off) and outlier rows sit at pool row page*P + t % P.
 // The length is also capped at npages[b] * P.  Scores, maximum and partials are those of BATCH.  Others ignore `pg`.
+// BITS = kVNPad3: the 3-bit kernel for a slab whose word rows are not a multiple of 8 -- one KV head, 12 rows.  One TMA
+// box of p.box_rows (16) rows stages them with the next rows of the tensor, which no unit reads: the next sequence's or
+// the next page's first rows of the same tokens, or TMA's zero fill past the tensor's last row.  Stages stay whole
+// 1024-byte swizzle atoms.  (A pseudo bit width rather than a PAD template argument, which would rename every
+// instantiation.)
 template <int BITS, bool SPLIT, bool GQA, bool BATCH, bool PAGED = false>
 __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_constant__ CUtensorMap tmap, const VNParams p,
                                                                 const int64_t bstride, const PageRef pg) {
-  using C = VNCfg<BITS>;
+  constexpr bool PAD = BITS == kVNPad3;
+  constexpr int NB = PAD ? 3 : BITS;
+  using C = VNCfg<NB>;
   constexpr int N = C::N, W = C::W, NP = C::NP, TABN = C::TABN;
   const int grp = GQA ? p.grp : 1;
   const int bz = BATCH ? (int)blockIdx.z : 0;
@@ -159,7 +167,7 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
   const int Hg = SPLIT ? p.H / (int)gridDim.y : p.H;     // heads of this CTA: [h0, h0 + Hg)
   const int h0 = SPLIT ? (int)blockIdx.y * Hg : 0;
   const int rows = Hg / grp * W;                          // word rows of the slab (KV heads)
-  const VNSmem lay = vn_smem_layout(rows, TABN, Hg, p.n_stages);
+  const VNSmem lay = vn_smem_layout(PAD ? p.box_rows : rows, TABN, Hg, p.n_stages);
   float2* s_tab = reinterpret_cast<float2*>(smem + lay.off_tab);   // [TABN][32 lanes]
   float* s_w = reinterpret_cast<float*>(smem + lay.off_w);         // [2][Hg][kNWStride]    w = exp(s - max)
   float* s_ws = reinterpret_cast<float*>(smem + lay.off_ws);       // [2][Hg][kNWsStride]   w * sf_t
@@ -169,10 +177,10 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
   const int S = p.n_stages;
   const int hidden = p.H * kHeadDim;
 
-  // ---- lane-private pair table: entry i -> {cent[i & (N-1)], cent[i >> BITS]} ---------------------------------
+  // ---- lane-private pair table: entry i -> {cent[i & (N-1)], cent[i >> BITS]} -------------------------------
   for (int i = tid; i < TABN * 32; i += kNThreads) {
     const int idx = i >> 5;
-    s_tab[i] = make_float2(p.v_cent[idx & (N - 1)], p.v_cent[(idx >> BITS) & (N - 1)]);
+    s_tab[i] = make_float2(p.v_cent[idx & (N - 1)], p.v_cent[(idx >> NB) & (N - 1)]);
   }
   const uint32_t tab = smem_u32(s_tab) + lane * 8;
 
@@ -180,7 +188,7 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
   int u_row[2], u_head[2], u_ch0[2], u_part[2];
   bool u_on[2];
   int sub = 0;
-  if constexpr (BITS == 3) {
+  if constexpr (NB == 3) {
     sub = warp % 3;
     const int tri = warp / 3;
     const int ngroups = Hg * 4;
@@ -199,7 +207,7 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
     for (int i = 0; i < 2; ++i) {
       const int u = tid + i * kNThreads;
       u_on[i] = u < nunits;
-      if constexpr (BITS == 4) { u_row[i] = u; u_part[i] = 0; u_head[i] = u >> 4; u_ch0[i] = (u & 15) * 8; }
+      if constexpr (NB == 4) { u_row[i] = u; u_part[i] = 0; u_head[i] = u >> 4; u_ch0[i] = (u & 15) * 8; }
       else { u_row[i] = u >> 1; u_part[i] = u & 1; u_head[i] = u >> 4; u_ch0[i] = ((u >> 1) & 7) * 16 + (u & 1) * 8; }
     }
   }
@@ -247,7 +255,7 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
   const int64_t tiles_per_cta = p.len_dev != nullptr ? (n_tiles_total + gridDim.x - 1) / gridDim.x : p.tiles_per_cta;
   const int64_t tile0 = (int64_t)blockIdx.x * tiles_per_cta;
   const int ntiles = (int)max((int64_t)0, min(tiles_per_cta, n_tiles_total - tile0));
-  const int nbox = rows / p.box_rows;
+  const int nbox = PAD ? 1 : rows / p.box_rows;
 
   auto issue_tile = [&](int it) {  // thread 0 only
     const int s = it % S;
@@ -389,12 +397,12 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
     for (int i = 0; i < 2; ++i) {
       if (u_on[i]) {
         const float* wsrow = wsbuf + u_head[i] * kNWsStride;
-        if constexpr (BITS == 3) {
+        if constexpr (NB == 3) {
           if (sub == 0) vn_tile_unit<3, 0>(stage, r_off[i], r_swz[i], r_off2[i], r_swz2[i], 0, tab, wsrow, acc[i]);
           else if (sub == 1) vn_tile_unit<3, 1>(stage, r_off[i], r_swz[i], r_off2[i], r_swz2[i], 0, tab, wsrow, acc[i]);
           else vn_tile_unit<3, 2>(stage, r_off[i], r_swz[i], r_off2[i], r_swz2[i], 0, tab, wsrow, acc[i]);
         } else {
-          vn_tile_unit<BITS, 0>(stage, r_off[i], r_swz[i], 0, 0, u_part[i], tab, wsrow, acc[i]);
+          vn_tile_unit<NB, 0>(stage, r_off[i], r_swz[i], 0, 0, u_part[i], tab, wsrow, acc[i]);
         }
       }
     }
@@ -443,7 +451,7 @@ __global__ void __launch_bounds__(kNThreads, 1) v_native_kernel(const __grid_con
   for (int i = 0; i < 2; ++i) {
     if (u_on[i]) {
       const float hoff = s_off[u_head[i]];
-      const int nch = (BITS == 3) ? (sub == 2 ? 10 : 11) : 8;
+      const int nch = (NB == 3) ? (sub == 2 ? 10 : 11) : 8;
 #pragma unroll
       for (int k = 0; k < 2 * NP; ++k) {
         if (k < nch) {
@@ -464,7 +472,7 @@ template <int BITS>
 static int vn_stages(int Hg, int grp, VNSmem* lay) {
   using C = VNCfg<BITS>;
   for (int S = kNMaxStages; S >= 2; --S) {
-    *lay = vn_smem_layout(Hg / grp * C::W, C::TABN, Hg, S);
+    *lay = vn_smem_layout((Hg / grp * C::W + 7) / 8 * 8, C::TABN, Hg, S);   // staged rows: whole 8-row atoms
     if (lay->total + 1024u <= kVNSmemBudget) return S;
   }
   return 0;
@@ -495,20 +503,27 @@ static int launch_vn(VNParams p, const AttendCall& c, const AttendScratch& s, in
   // G head groups: 1 while the whole slab fits (every shape up to 4-bit H = 32, 3-bit H = 56, 2-bit H = 64), else 2.
   // G = 2 always fits for H <= 64: Hg = H/2 <= 32 heads is at most the 7B slab, and H % 4 == 0 keeps Hg even, so
   // the 3-bit group rows (Hg*12) stay a multiple of 8 for the TMA box below.
-  // GQA: the slab holds H/grp KV heads, and each of the G = 2 groups whole KV-head groups (H/grp % 4 == 0).
+  // GQA: the slab holds H/grp KV heads, and each of the G = 2 groups whole KV-head groups (H/grp % 4 == 0).  One or two
+  // KV heads are a slab of at most 32 rows, which always fits whole (G = 1).
   VNSmem lay{};
   int G = 1;
   int S = vn_stages<BITS>(p.H, p.grp, &lay);
   if (S < 2) { G = 2; S = vn_stages<BITS>(p.H / G, p.grp, &lay); }
-  if (S < 2) return KVQ_E_UNSUPPORTED;
+  if (S < 2 || (G == 2 && (p.H / p.grp) % 4 != 0)) return KVQ_E_UNSUPPORTED;
   p.n_stages = S;
   const int rows = p.H / G / p.grp * C::W;   // word rows of one head group
   CUtensorMap tmap;
   // largest TMA box height <= 256 that divides the group's row count (a multiple of 8); one map over the whole
-  // cache, the kernel offsets the row coordinate by its group's first row
-  int nb = (rows + 255) / 256;
-  while (rows % nb != 0 || (rows / nb) % 8 != 0) ++nb;
-  p.box_rows = rows / nb;
+  // cache, the kernel offsets the row coordinate by its group's first row.  One 3-bit KV head (12 rows): one box of 16
+  // rows, the kVNPad3 kernel.
+  const bool pad = rows % 8 != 0;
+  if (pad) {
+    p.box_rows = (rows + 7) / 8 * 8;
+  } else {
+    int nb = (rows + 255) / 256;
+    while (rows % nb != 0 || (rows / nb) % 8 != 0) ++nb;
+    p.box_rows = rows / nb;
+  }
   // a batch: one map over the B sequences' caches (sequence b's rows follow b*Hkv*W others); a paged batch: one map
   // over the pool (n_pool*Hkv*W rows of P tokens)
   int rc = paged
@@ -526,6 +541,8 @@ static int launch_vn(VNParams p, const AttendCall& c, const AttendScratch& s, in
   const uint32_t smem = lay.total + 1024u;
   const PageRef pg = paged ? *c.pg : PageRef{};
   rc = with_flavour(p.grp > 1, batch, paged, [&](auto GQA, auto BATCH, auto PAGED) {
+    if constexpr (BITS == 3 && GQA())   // (pad implies one 3-bit KV head under GQA, G = 1)
+      if (pad) return launch_vn_kernel<kVNPad3, false, true, BATCH(), PAGED()>(tmap, p, grid, smem, c.stream, s.bstride, pg);
     return G == 1 ? launch_vn_kernel<BITS, false, GQA(), BATCH(), PAGED()>(tmap, p, grid, smem, c.stream, s.bstride, pg)
                   : launch_vn_kernel<BITS, true, GQA(), BATCH(), PAGED()>(tmap, p, grid, smem, c.stream, s.bstride, pg);
   });
