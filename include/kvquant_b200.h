@@ -524,6 +524,70 @@ KVQ_API int kvq_attend_chunk_gqa(int bits, int Hq, int Hkv, int64_t Lmax, int64_
                    float* out, void* scratch, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Ragged prefill (DESIGN.md section 4.15): the chunks of several slots of a batch appended, or attended, in one launch.
+ * The slots are described by a HOST segment table segs int64 [n_seg][4] of (slot b, first slot s0, T, first row):
+ * segment i covers rows row0 .. row0 + T - 1 of the packed inputs and slots s0 .. s0 + T - 1 of slot b.  Rows are
+ * packed in segment order (row0 = the sum of the earlier segments' T, N = the sum of all), the slots are distinct and
+ * T may be 0 (nothing written or attended).  The table is read on the host and passed to the kernels by value.
+ *   Contiguous forms: the cache tensors are the batch-strided ones of kvq_append_kv_fused_batch / kvq_attend_batch
+ *     (kcache [B, Hkv, W, Lmax], vlut [B, Lmax, 2^bits], v_aff [B, Lmax, 2], outlier rows [B, Lmax, n_out]).
+ *   Paged forms: the page pools and batch page table (device int32 [B, max_pages]) of kvq_append_kv_fused_paged, and
+ *     n_mapped, a HOST int32 [n_seg]: how many leading entries of segment i's table row are mapped.
+ *   kvq_append_kv_fused_chunk_ragged[_paged]: k_new, v_new f32 [N, Hkv*128]; every segment's slots are left bit for bit
+ *     as kvq_append_kv_fused_chunk[_paged] of that segment alone leaves them; no other slot is written.  One launch.
+ *   kvq_attend_chunk_ragged[_paged]: q f32 [N, Hq, 128], row j of segment i rotated at pos_offset + s0_i + j; chunk_k /
+ *     chunk_v f16 [Hkv, N, 128] (the segments' rotated keys and values); sinks per slot, sink_k f16 [B, Hkv, 128, n_sink]
+ *     and sink_v f16 [B, Hkv, n_sink, 128]; one rope table covering [0, pos_offset + max s0).  Segment i attends over
+ *     slot b_i's sinks, its first s0_i slots and its own rows causally: its output rows are bit for bit those of
+ *     kvq_attend_chunk_gqa on that slot with L = s0_i (same split count, same merge order).  scratch: a device buffer of
+ *     kvq_attend_chunk_ragged_scratch_bytes(Hq, n_seg, segs) bytes (0 for an invalid table).  One launch, two when a
+ *     segment splits.
+ *   Checks, all before any device access: each entry point's single-sequence checks with their codes and order (the
+ *   page geometry first for the paged forms), where after the size checks 1 <= B <= 256, 0 <= n_seg <= B and N >= 0
+ *   (KVQ_E_SHAPE), segs == NULL with n_seg > 0 or a paged n_mapped == NULL (KVQ_E_NULL), then the table: a slot outside
+ *   [0, B) or named twice, s0 or T negative, rows not packed in order, s0 + T past the per-slot cap (Lmax, or
+ *   max_pages * P), n_mapped[i] outside [0, max_pages], the slots touched not mapped (s0 + T for the appends, which
+ *   write them; s0 for the attends, which read the first s0), their sum not N, or N >= 2^31 -> KVQ_E_SHAPE; the attends
+ *   then check rope_npos against the largest s0.  N == 0 returns 0 once these hold, whatever the data pointers, and launches nothing.
+ * ------------------------------------------------------------------------------------------------------------- */
+KVQ_API int kvq_append_kv_fused_chunk_ragged(int bits, int B, int H, int64_t Lmax, int n_seg, const int64_t* segs,
+                              int64_t N, int n_each,
+                              const float* k_new, int32_t* kcache, const float* klut, const float* klut_sub,
+                              const float* k_thr_lower, const float* k_thr_upper,
+                              float* k_outliers, int32_t* k_outlier_idx,
+                              const float* v_new, int32_t* vcache, const float* v_cent, const float* v_cent_deq,
+                              float* vlut_tok, float* v_aff,
+                              float* v_outliers, int32_t* v_outlier_idx,
+                              void* stream);
+KVQ_API int kvq_append_kv_fused_chunk_ragged_paged(int bits, int B, int H, int n_pool, int n_seg, const int64_t* segs,
+                              int64_t N, int n_each,
+                              const float* k_new, int32_t* kcache, const float* klut, const float* klut_sub,
+                              const float* k_thr_lower, const float* k_thr_upper,
+                              float* k_outliers, int32_t* k_outlier_idx,
+                              const float* v_new, int32_t* vcache, const float* v_cent, const float* v_cent_deq,
+                              float* vlut_tok, float* v_aff,
+                              float* v_outliers, int32_t* v_outlier_idx,
+                              void* stream, const int32_t* page_table, int max_pages, const int32_t* n_mapped, int P);
+KVQ_API int64_t kvq_attend_chunk_ragged_scratch_bytes(int Hq, int n_seg, const int64_t* segs);
+KVQ_API int kvq_attend_chunk_ragged(int bits, int B, int Hq, int Hkv, int64_t Lmax, int n_seg, const int64_t* segs,
+                   int64_t N, const float* q, const void* chunk_k, const void* chunk_v,
+                   const int32_t* kcache, const float* klut, const float* k_outliers, const int32_t* k_outlier_idx,
+                   const int32_t* vcache, const float* v_cent, const float* v_aff,
+                   const float* v_outliers, const int32_t* v_outlier_idx, int n_out,
+                   const float* rope_cos_sin, int64_t rope_npos, int pos_offset,
+                   const void* sink_k, const void* sink_v, int n_sink,
+                   float* out, void* scratch, void* stream);
+KVQ_API int kvq_attend_chunk_ragged_paged(int bits, int B, int Hq, int Hkv, int n_pool, int n_seg, const int64_t* segs,
+                   int64_t N, const float* q, const void* chunk_k, const void* chunk_v,
+                   const int32_t* kcache, const float* klut, const float* k_outliers, const int32_t* k_outlier_idx,
+                   const int32_t* vcache, const float* v_cent, const float* v_aff,
+                   const float* v_outliers, const int32_t* v_outlier_idx, int n_out,
+                   const float* rope_cos_sin, int64_t rope_npos, int pos_offset,
+                   const void* sink_k, const void* sink_v, int n_sink,
+                   float* out, void* scratch, void* stream,
+                   const int32_t* page_table, int max_pages, const int32_t* n_mapped, int P);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Uncapped "orig" sparse path, 4-bit only (quant_cuda.cpp:347-399).
  * SpMV halves of ..._opt2_orig: balanced CSR (K; rows = tokens) quant_cuda_kernel.cu:523-614 and CSC (V; cols =
  * tokens) 616-689; the dense half is kvq_k_matvec / kvq_v_matvec with outliers == NULL.

@@ -92,6 +92,18 @@ SIGNATURES = {
                                   _p, _c_int, _p, _c_i64, _c_int, _p, _p, _c_int, _p, _p, _p]),
     "kvq_attend_chunk_gqa": (_c_int, [_c_int, _c_int, _c_int, _c_i64, _c_i64, _c_i64, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                       _p, _p, _p, _c_int, _p, _c_i64, _c_int, _p, _p, _c_int, _p, _p, _p]),
+    "kvq_append_kv_fused_chunk_ragged": (_c_int, [_c_int, _c_int, _c_int, _c_i64, _c_int, _p, _c_i64, _c_int, _p, _p,
+                                                  _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "kvq_append_kv_fused_chunk_ragged_paged": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _p, _c_i64, _c_int,
+                                                        _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
+                                                        _p, _p, _p, _c_int, _p, _c_int]),
+    "kvq_attend_chunk_ragged_scratch_bytes": (_c_i64, [_c_int, _c_int, _p]),
+    "kvq_attend_chunk_ragged": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_i64, _c_int, _p, _c_i64, _p, _p, _p, _p,
+                                         _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _p, _c_i64, _c_int, _p, _p, _c_int, _p,
+                                         _p, _p]),
+    "kvq_attend_chunk_ragged_paged": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _p, _c_i64, _p, _p, _p,
+                                               _p, _p, _p, _p, _p, _p, _p, _p, _p, _c_int, _p, _c_i64, _c_int, _p, _p,
+                                               _c_int, _p, _p, _p, _p, _c_int, _p, _c_int]),
     "kvq_p2p_buffer_bytes": (_c_i64, [_c_int, _c_int]),
     "kvq_p2p_alloc": (_c_int, [_p, _c_i64, _p]),
     "kvq_p2p_open": (_c_int, [_p, _p]),

@@ -547,16 +547,19 @@ class LayerCache:
             raise ValueError("k and v must be [%d, %d]" % (T, self.hidden))
         return T
 
-    def _chunk_kv16(self, k, v, rope_theta, p0, out_k, out_v):
+    def _chunk_kv16(self, k, v, rope_theta, p0, out_k, out_v, npos=None):
         """The chunk's keys rotated at positions p0 + i and its values, written as fp16 into out_k / out_v [H, T, 128]
         (views allowed): the chunk operands both chunk attentions use.  Returns the f32 rope table, covering
-        p0 + T positions."""
+        p0 + T positions.  p0 may instead be an int64 device tensor [T] of per-row positions, all below npos (the rows
+        of several slots' chunks, _BatchCommon.attend_chunks); row i is then rotated at p0[i], with the same values."""
         T = k.shape[0]
+        rows = isinstance(p0, torch.Tensor)
         if isinstance(rope_theta, RopeLenState):
             rope, _ = self._table(rope_theta)
         else:
-            rope, _, _ = qc.rope_tables(self.device, rope_theta, p0 + T)
-        cos, sin = rope[:, p0:p0 + T, 0].t()[:, None, :], rope[:, p0:p0 + T, 1].t()[:, None, :]   # [T, 1, 64]
+            rope, _, _ = qc.rope_tables(self.device, rope_theta, npos if rows else p0 + T)
+        tab = rope[:, p0] if rows else rope[:, p0:p0 + T]                                          # [64, T, 2]
+        cos, sin = tab[..., 0].t()[:, None, :], tab[..., 1].t()[:, None, :]                         # [T, 1, 64]
         kc = k.view(T, self.H, HEAD_DIM)
         lo, hi = kc[..., :HEAD_DIM // 2], kc[..., HEAD_DIM // 2:]
         out_k[:, :, :HEAD_DIM // 2] = (cos * lo - sin * hi).transpose(0, 1)
@@ -741,6 +744,7 @@ class _BatchCommon:
 
     # the entry points and their extra arguments (overridden by the paged cache)
     _append_fn, _attend_fn = "kvq_append_kv_fused_batch", "kvq_attend_batch"
+    _append_chunks_fn, _attend_chunks_fn = "kvq_append_kv_fused_chunk_ragged", "kvq_attend_chunk_ragged"
 
     def _page_args(self):
         return ()
@@ -816,6 +820,115 @@ class _BatchCommon:
         _lib.check(getattr(self.lib, self._attend_fn + sfx)(*args), self._attend_fn + sfx)
         return out
 
+    # -- several slots' chunks in one launch (ragged prefill, DESIGN.md section 4.15) ------------------------------------
+    def _segments(self, slots, starts, counts, N):
+        """The host segment table int64 [n_seg, 4] of (slot, s0, T, first row) after the checks a caller can fail:
+        slots distinct and in range, counts >= 0 summing to N (ValueError), s0 + T within the cap (IndexError)."""
+        slots, counts = [int(b) for b in slots], [int(t) for t in counts]
+        if len(slots) != len(counts):
+            raise ValueError("%d slots but %d counts" % (len(slots), len(counts)))
+        if len(set(slots)) != len(slots):
+            raise ValueError("slots must be distinct, got %s" % (slots,))
+        for b in slots:
+            if not 0 <= b < self.B:
+                raise IndexError("slot %d out of range [0, %d)" % (b, self.B))
+        if any(t < 0 for t in counts) or sum(counts) != N:
+            raise ValueError("counts must be >= 0 and sum to the %d rows, got %s" % (N, counts))
+        for b, s0, t in zip(slots, starts, counts):
+            if s0 + t > self.Lmax:
+                raise IndexError("a chunk of %d tokens does not fit slot %d: %d of %d slots used" % (t, b, s0, self.Lmax))
+        row0 = np.concatenate(([0], np.cumsum(counts)[:-1])) if counts else np.zeros(0)
+        return np.ascontiguousarray(np.stack([np.asarray(slots), np.asarray(starts), np.asarray(counts), row0], axis=1)
+                                    .astype(np.int64).reshape(-1, 4))
+
+    def _map_chunks(self, slots, starts, counts):
+        """Paged: map the pages the segments' writes need, after checking them all (contiguous: nothing to do)."""
+
+    def _chunks_tail(self, slots):
+        """The trailing arguments of the ragged entry points (contiguous: none)."""
+        return ()
+
+    @_on_cache_device
+    def _append_chunks_at(self, slots, starts, k, v, counts):
+        """append_chunks at the given first slots, host lengths untouched."""
+        c = self._tmpl
+        if k.dim() != 2 or tuple(k.shape) != tuple(v.shape) or k.shape[1] != self.hidden:
+            raise ValueError("k and v must both be [N, %d], got %s and %s" % (self.hidden, tuple(k.shape), tuple(v.shape)))
+        N = k.shape[0]
+        kp, vp = c._vec(k, N * self.hidden, "k"), c._vec(v, N * self.hidden, "v")
+        segs = self._segments(slots, starts, counts, N)
+        self._map_chunks(segs[:, 0].tolist(), segs[:, 1].tolist(), segs[:, 2].tolist())
+        if N == 0:
+            return
+        tail, fn = self._chunks_tail(segs[:, 0].tolist()), self._append_chunks_fn
+        _lib.check(getattr(self.lib, fn)(
+            self.bits, self.B, self.H, self._extent, len(segs), segs.ctypes.data, N, self.n_each,
+            kp, self.kcache.data_ptr(), c.klut.data_ptr(), c.klut_sub.data_ptr(), c.thr_lower.data_ptr(),
+            c.thr_upper.data_ptr(), *self._ptrs("k"), vp, self.vcache.data_ptr(), c.v_cent.data_ptr(),
+            c.v_cent_deq.data_ptr() if c.v_norm is not None else None, self.vlut.data_ptr(), self.vaff.data_ptr(),
+            *self._ptrs("v"), torch.cuda.current_stream().cuda_stream, *tail), fn)
+
+    def append_chunks(self, slots, k, v, counts):
+        """append_chunk of several slots in one launch (kvq_append_kv_fused_chunk_ragged[_paged]): k, v f32 [N, hidden]
+        hold counts[i] rows for slots[i], in that order; slot b's rows go to its slots host_len(b) onwards, bit for bit
+        as append_chunk of those rows alone.  Slots must be distinct; a count of 0 writes nothing.  Past the cap raises
+        IndexError, and (paged) an exhausted pool RuntimeError, before anything is written or reserved for any slot.
+        Advances the host lengths; commit(*slots) publishes them to the device."""
+        starts = [self._host_len(b) for b in slots]
+        self._append_chunks_at(slots, starts, k, v, counts)
+        for b, t in zip(slots, counts):
+            self._set_host_len(b, self._host_len(b) + int(t))
+
+    @_on_cache_device
+    def _attend_chunks_at(self, slots, starts, q, k, v, counts, rope):
+        """attend_chunks with the given cached lengths; rope: a resolved rotation (theta or RotarySpec)."""
+        c = self._tmpl
+        if c.group > 1:
+            c._gqa_check()
+        if not c.use_native_v:
+            raise NotImplementedError("attend_chunks reads the native V form (use_native_v=True)")
+        if isinstance(rope, (LengthDependentRotary, RopeLenState)):
+            raise NotImplementedError("attend_chunks with length-dependent rotary frequencies: each slot needs its own "
+                                      "frequency table; prefill such slots one at a time (prefill_seq)")
+        if q.dim() != 3 or q.shape[1:] != (self.Hq, HEAD_DIM):
+            raise ValueError("q must be [N, %d, %d], got %s" % (self.Hq, HEAD_DIM, tuple(q.shape)))
+        N = q.shape[0]
+        for t, name, n in ((q, "q", self.q_hidden), (k, "k", self.hidden), (v, "v", self.hidden)):
+            c._vec(t, N * n, name)
+        if tuple(k.shape) != (N, self.hidden) or tuple(v.shape) != (N, self.hidden):
+            raise ValueError("k and v must be [%d, %d]" % (N, self.hidden))
+        segs = self._segments(slots, starts, counts, N)
+        out = torch.empty((N, self.Hq, HEAD_DIM), dtype=torch.float32, device=self.device)
+        if N == 0:
+            return out
+        # row j of segment i sits at n_sink + s0_i + j
+        pos = np.concatenate([np.arange(s0, s0 + t) for s0, t in zip(segs[:, 1], segs[:, 2])]) + self.n_sink
+        kc = torch.empty((self.H, N, HEAD_DIM), dtype=torch.float16, device=self.device)
+        vc = torch.empty_like(kc)
+        tab = c._chunk_kv16(k, v, rope, torch.from_numpy(pos).to(self.device), kc, vc, npos=int(pos.max()) + 1)
+        scratch = torch.empty(max(self.lib.kvq_attend_chunk_ragged_scratch_bytes(self.Hq, len(segs), segs.ctypes.data),
+                                  16), dtype=torch.uint8, device=self.device)
+        ns = self.n_sink if self.sink_k is not None else 0
+        tail, fn = self._chunks_tail(segs[:, 0].tolist()), self._attend_chunks_fn
+        _lib.check(getattr(self.lib, fn)(
+            self.bits, self.B, self.Hq, self.H, self._extent, len(segs), segs.ctypes.data, N, q.data_ptr(),
+            kc.data_ptr(), vc.data_ptr(), self.kcache.data_ptr(), c.klut_deq.data_ptr(), *self._ptrs("k"),
+            self.vcache.data_ptr(), c.v_cent_deq.data_ptr(), self.vaff.data_ptr(), *self._ptrs("v"), self.n_out,
+            tab.data_ptr(), tab.shape[1], self.n_sink, self.sink_k.data_ptr() if ns else None,
+            self.sink_v.data_ptr() if ns else None, ns, out.data_ptr(), scratch.data_ptr(),
+            torch.cuda.current_stream().cuda_stream, *tail), fn)
+        return out
+
+    def attend_chunks(self, slots, q, k, v, counts, rope_theta=10000.0, rope=None):
+        """attend_chunk_fused of several slots in one launch (kvq_attend_chunk_ragged[_paged]): q f32 [N, q_heads, 128]
+        and k, v f32 [N, hidden] hold counts[i] rows for slots[i], in that order, row j of slot b's rows rotated at
+        n_sink + host_len(b) + j.  Each slot's rows attend over its sinks, its host_len(b) cached tokens and its own rows
+        causally, and come out bit for bit as attend_chunk_fused of those rows alone on that slot.  Returns f32
+        [N, q_heads, 128]; the cache is not modified.  rope: theta or a static RotarySpec (length-dependent rotary
+        raises NotImplementedError), as attend_chunk_fused's."""
+        starts = [self._host_len(b) for b in slots]
+        return self._attend_chunks_at(slots, starts, q, k, v, counts, _resolve(rope, rope_theta))
+
 
 class BatchedLayerCache(_BatchCommon):
     """One layer's quantised cache for B sequences (batched decode, DESIGN.md section 4.10).
@@ -880,6 +993,12 @@ class BatchedLayerCache(_BatchCommon):
     @property
     def lens_host(self):
         return [v.len for v in self._views]
+
+    def _host_len(self, b):
+        return self._views[b].len
+
+    def _set_host_len(self, b, n):
+        self._views[b].len = n
 
     def commit(self, *slots):
         """Copy the host lengths (the views' `len`) of the given slots -- every slot when none is given -- to the
@@ -1049,6 +1168,7 @@ class PagedLayerCache(_BatchCommon):
     load_seq(b, lc, n) pages a contiguous cache's first n slots in and read_seq(b, lc) pages slot b out into one."""
 
     _append_fn, _attend_fn = "kvq_append_kv_fused_paged", "kvq_attend_paged"
+    _append_chunks_fn, _attend_chunks_fn = "kvq_append_kv_fused_chunk_ragged_paged", "kvq_attend_chunk_ragged_paged"
 
     def __init__(self, batch, bits, num_heads, klut, klut_sub, thr_lower, thr_upper, v_cent, device,
                  include_sparse=True, sparsity_threshold=0.99, n_sink=0, v_norm=None, sparse_v=None, q_heads=None,
@@ -1110,6 +1230,34 @@ class PagedLayerCache(_BatchCommon):
     @property
     def lens_host(self):
         return list(self.pages.lens_host)
+
+    def _host_len(self, b):
+        return self.pages.lens_host[self.pages._slot(b)]
+
+    def _set_host_len(self, b, n):
+        self.pages.lens_host[b] = n
+
+    def _map_chunks(self, slots, starts, counts):
+        """Check every segment's write range against the shared-page rule and the pool's free pages, then map them:
+        a refusal (RuntimeError) leaves the table as it was for every slot."""
+        pg = self.pages
+        need = 0
+        for b, s0, t in zip(slots, starts, counts):
+            if t == 0:
+                continue
+            shared = [p for p in pg.pages[b][s0 // self.P:-(-(s0 + t) // self.P)] if pg.refs[p] > 1]
+            if shared:
+                raise RuntimeError("slots [%d, %d) of slot %d lie in shared pages %s" % (s0, s0 + t, b, shared))
+            need += max(0, -(-(s0 + t) // self.P) - len(pg.pages[b]))
+        if need > pg.n_free:
+            raise RuntimeError("page pool exhausted: %d pages needed, %d of %d free" % (need, pg.n_free, self.n_pool))
+        for b, s0, t in zip(slots, starts, counts):
+            pg.reserve(b, s0 + t)
+
+    def _chunks_tail(self, slots):
+        pg = self.pages
+        self._n_mapped = np.asarray([len(pg.pages[b]) for b in slots], dtype=np.int32)   # (alive through the call)
+        return (pg.table.data_ptr(), pg.max_pages, self._n_mapped.ctypes.data, pg.P)
 
     def commit(self, *slots):
         """Copy the host lengths of the given slots -- every slot when none is given -- to the device lengths."""

@@ -62,7 +62,14 @@ struct Params {
   int H, n_out, nsplit;              // H: query heads
   int grp;                           // query heads per KV head: query head h reads KV head h / grp
   int64_t Lmax, L, T, tiles_per_split;
+  // ragged forms only (chunk_attend_ragged_kernel): rows per KV head of ck / cv, and a paged slot's page-table row
+  int64_t cstride;
+  const int32_t* pages; int P;
 };
+
+// FORM 0: one sequence of a contiguous cache (chunk_attend_kernel); 1: a segment of a contiguous batch, 2: a segment
+// of a page pool (chunk_attend_ragged_kernel: Params rebased on the segment, ck / cv rows cstride apart per KV head)
+constexpr int kLone = 0, kRagged = 1, kRaggedPaged = 2;
 
 __device__ __forceinline__ void cp_async4(void* dst, const void* src, bool valid) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(valid ? 4 : 0)
@@ -91,8 +98,9 @@ struct Tiles {
   __device__ int64_t count() const { return n_sink + n_slot + n_chunk; }
 };
 
-// cp.async the packed K/V words and (sf, off) of slot tile `st` into buffer `b`; rows past L are zero-filled
-template <int BITS>
+// cp.async the packed K/V words and (sf, off) of slot tile `st` into buffer `b`; rows past L are zero-filled.
+// kRaggedPaged: each token's words through its own page (64-token tiles straddle pages of 160 * k tokens)
+template <int BITS, int FORM>
 __device__ __forceinline__ void prefetch_slot(const Params& p, unsigned char* smem, int64_t st, int b, int h) {
   using S = Smem<BITS>;
   constexpr int W = S::W;
@@ -101,21 +109,39 @@ __device__ __forceinline__ void prefetch_slot(const Params& p, unsigned char* sm
   float* aff = reinterpret_cast<float*>(smem + S::oAff) + b * 2 * kBK;
   const int64_t t0 = st * kBK;
   const int nt = (int)min((int64_t)kBK, p.L - t0);
-  for (int i = threadIdx.x; i < W * kBK; i += kThreads) {
-    const int r = i / kBK, t = i % kBK;             // t fastest: coalesced along the sequence
+  if constexpr (FORM == kRaggedPaged) {
+    const PageRef pr{p.pages, nullptr, 0, p.P, 0};
+    const int t = threadIdx.x % kBK;                // kThreads % kBK == 0: a thread keeps its token
     const bool ok = t < nt;
-    const int64_t g = ((int64_t)h * W + r) * p.Lmax + t0 + (ok ? t : 0);
-    cp_async4(wk + t * S::kWP + r, p.kcache + g, ok);
-    cp_async4(wv + t * S::kWP + r, p.vcache + g, ok);
-  }
-  if (threadIdx.x < 2 * kBK) {
-    const bool ok = (int)threadIdx.x < 2 * nt;
-    cp_async4(aff + threadIdx.x, p.vaff + 2 * t0 + (ok ? threadIdx.x : 0), ok);
+    const PageCol pc = page_col(pr, (int)(t0 + (ok ? t : 0)));
+    const int64_t g0 = ((int64_t)pc.page * (p.H / p.grp) + h) * W * p.P + pc.col;   // pool [page][Hkv][W][P]
+    for (int r = threadIdx.x / kBK; r < W; r += kThreads / kBK) {
+      cp_async4(wk + t * S::kWP + r, p.kcache + g0 + (int64_t)r * p.P, ok);
+      cp_async4(wv + t * S::kWP + r, p.vcache + g0 + (int64_t)r * p.P, ok);
+    }
+    if (threadIdx.x < 2 * kBK) {
+      const int tt = threadIdx.x >> 1;
+      const bool oka = tt < nt;
+      cp_async4(aff + threadIdx.x, p.vaff + 2 * page_row(pr, (int)(t0 + (oka ? tt : 0))) + (threadIdx.x & 1), oka);
+    }
+  } else {
+    for (int i = threadIdx.x; i < W * kBK; i += kThreads) {
+      const int r = i / kBK, t = i % kBK;           // t fastest: coalesced along the sequence
+      const bool ok = t < nt;
+      const int64_t g = ((int64_t)h * W + r) * p.Lmax + t0 + (ok ? t : 0);
+      cp_async4(wk + t * S::kWP + r, p.kcache + g, ok);
+      cp_async4(wv + t * S::kWP + r, p.vcache + g, ok);
+    }
+    if (threadIdx.x < 2 * kBK) {
+      const bool ok = (int)threadIdx.x < 2 * nt;
+      cp_async4(aff + threadIdx.x, p.vaff + 2 * t0 + (ok ? threadIdx.x : 0), ok);
+    }
   }
 }
 
-template <int BITS>
-__global__ void __launch_bounds__(kThreads, 1) chunk_attend_kernel(const Params p) {
+// CTA (query block qb, head h, key split s) of the call (or segment) p; the lone kernel reads them from its grid
+template <int BITS, int FORM>
+__device__ __forceinline__ void chunk_attend_body(const Params& p, int64_t qb_r, int h_r, int s_r) {
   using S = Smem<BITS>;
   constexpr int W = S::W;
   constexpr int WQ = W / 4;
@@ -129,8 +155,8 @@ __global__ void __launch_bounds__(kThreads, 1) chunk_attend_kernel(const Params 
   float* cent = reinterpret_cast<float*>(smem + S::oCent);
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t qb = blockIdx.x;
-  const int h = blockIdx.y, s = blockIdx.z, H = p.H;
+  const int64_t qb = FORM == kLone ? (int64_t)blockIdx.x : qb_r;
+  const int h = FORM == kLone ? (int)blockIdx.y : h_r, s = FORM == kLone ? (int)blockIdx.z : s_r, H = p.H;
   const int hk = h / p.grp;                           // the KV head: LUT, words, (sf, off), outliers, sinks, chunk K/V
   const int64_t T = p.T, L = p.L;
   const int64_t row0 = qb * kBQ;                      // first query row of the block
@@ -143,7 +169,7 @@ __global__ void __launch_bounds__(kThreads, 1) chunk_attend_kernel(const Params 
   tl.n_chunk = s == 0 ? (min(T, row0 + kBQ) + kBK - 1) / kBK : 0;   // chunk tiles wholly after the last row: skipped
   const int64_t n_tiles = tl.count();
 
-  if (tl.n_sink == 0 && tl.n_slot > 0) prefetch_slot<BITS>(p, smem, tl.s0, 0, hk);
+  if (tl.n_sink == 0 && tl.n_slot > 0) prefetch_slot<BITS, FORM>(p, smem, tl.s0, 0, hk);
   cp_async_commit();
 
   // Q of the block, rounded to fp16 once, staged over the fp32 tiles, then held in registers as A fragments
@@ -181,7 +207,7 @@ __global__ void __launch_bounds__(kThreads, 1) chunk_attend_kernel(const Params 
   for (int64_t j = 0; j < n_tiles; ++j) {
     // next slot tile's words on their way while this tile is produced and consumed
     const int64_t jn = j + 1 - tl.n_sink;
-    if (jn >= 0 && jn < tl.n_slot) prefetch_slot<BITS>(p, smem, tl.s0 + jn, (int)(jn & 1), hk);
+    if (jn >= 0 && jn < tl.n_slot) prefetch_slot<BITS, FORM>(p, smem, tl.s0 + jn, (int)(jn & 1), hk);
     cp_async_commit();
     cp_async_wait_1();
     __syncthreads();                                  // words of tile j landed; Ks / Vs free
@@ -218,15 +244,31 @@ __global__ void __launch_bounds__(kThreads, 1) chunk_attend_kernel(const Params 
       if (p.kout != nullptr || p.vout != nullptr) {
         __syncthreads();
         const int64_t r0 = t0 * p.n_out;
-        for (int i = tid; i < nv * p.n_out; i += kThreads) {
-          const int t = i / p.n_out;
-          if (p.kout != nullptr) {
-            const int idx = p.kidx[r0 + i];
-            if ((idx >> 7) == hk) dq_add_outlier(&stK[t * kFP + (idx & 127)], p.kout[r0 + i]);
+        if constexpr (FORM == kRaggedPaged) {         // the same, each token's row through its page
+          const PageRef pr{p.pages, nullptr, 0, p.P, 0};
+          for (int i = tid; i < nv * p.n_out; i += kThreads) {
+            const int t = i / p.n_out;
+            const int64_t e = page_row(pr, (int)(t0 + t)) * p.n_out + (i - t * p.n_out);
+            if (p.kout != nullptr) {
+              const int idx = p.kidx[e];
+              if ((idx >> 7) == hk) dq_add_outlier(&stK[t * kFP + (idx & 127)], p.kout[e]);
+            }
+            if (p.vout != nullptr) {
+              const int idx = p.vidx[e];
+              if ((idx >> 7) == hk) dq_add_outlier(&stV[t * kFP + (idx & 127)], p.vout[e]);
+            }
           }
-          if (p.vout != nullptr) {
-            const int idx = p.vidx[r0 + i];
-            if ((idx >> 7) == hk) dq_add_outlier(&stV[t * kFP + (idx & 127)], p.vout[r0 + i]);
+        } else {
+          for (int i = tid; i < nv * p.n_out; i += kThreads) {
+            const int t = i / p.n_out;
+            if (p.kout != nullptr) {
+              const int idx = p.kidx[r0 + i];
+              if ((idx >> 7) == hk) dq_add_outlier(&stK[t * kFP + (idx & 127)], p.kout[r0 + i]);
+            }
+            if (p.vout != nullptr) {
+              const int idx = p.vidx[r0 + i];
+              if ((idx >> 7) == hk) dq_add_outlier(&stV[t * kFP + (idx & 127)], p.vout[r0 + i]);
+            }
           }
         }
       }
@@ -252,7 +294,7 @@ __global__ void __launch_bounds__(kThreads, 1) chunk_attend_kernel(const Params 
         const int t = i / (kHeadDim / 8), c0 = (i % (kHeadDim / 8)) * 8;
         uint4 ko = make_uint4(0u, 0u, 0u, 0u), vo = ko;
         if (t < nv) {
-          const int64_t off = ((int64_t)hk * T + chunk0 + t) * kHeadDim + c0;
+          const int64_t off = ((int64_t)hk * (FORM == kLone ? T : p.cstride) + chunk0 + t) * kHeadDim + c0;
           ko = *reinterpret_cast<const uint4*>(p.ck + off);
           vo = *reinterpret_cast<const uint4*>(p.cv + off);
         }
@@ -358,11 +400,14 @@ __global__ void __launch_bounds__(kThreads, 1) chunk_attend_kernel(const Params 
   }
 }
 
-// out[row, h] = sum_s 2^(m_s - M) O_s / sum_s 2^(m_s - M) l_s, splits taken in order
-__global__ void __launch_bounds__(kHeadDim) chunk_combine_kernel(const float* __restrict__ part, float* __restrict__ out,
-                                                                 int64_t TH, int nsplit) {
-  const int64_t rh = blockIdx.x;
-  const int d = threadIdx.x;
+template <int BITS>
+__global__ void __launch_bounds__(kThreads, 1) chunk_attend_kernel(const Params p) {
+  chunk_attend_body<BITS, kLone>(p, 0, 0, 0);
+}
+
+// out[row, h] = sum_s 2^(m_s - M) O_s / sum_s 2^(m_s - M) l_s, splits taken in order; (row, head) rh, channel d
+__device__ __forceinline__ void combine_row(const float* __restrict__ part, float* __restrict__ out, int64_t TH,
+                                            int nsplit, int64_t rh, int d) {
   float M = -INFINITY;
   for (int s = 0; s < nsplit; ++s) M = fmaxf(M, part[(s * TH + rh) * kPart + kHeadDim]);
   float num = 0.f, den = 0.f;
@@ -373,6 +418,77 @@ __global__ void __launch_bounds__(kHeadDim) chunk_combine_kernel(const float* __
     den = fmaf(w, ps[kHeadDim + 1], den);
   }
   out[rh * kHeadDim + d] = num / den;
+}
+
+__global__ void __launch_bounds__(kHeadDim) chunk_combine_kernel(const float* __restrict__ part, float* __restrict__ out,
+                                                                 int64_t TH, int nsplit) {
+  combine_row(part, out, TH, nsplit, blockIdx.x, threadIdx.x);
+}
+
+// ---- ragged chunk attend (kvq_attend_chunk_ragged[_paged], DESIGN.md section 4.15) ------------------------------------
+// Several slots' chunks in one launch: segment i attends its T rows over slot b's sinks, its first L (= s0) quantised
+// slots and its own rows, with the split count the lone call would choose for (T, L).  Grid (sum of the segments'
+// query blocks x splits, H): segment i owns x in [cta0[i], cta0[i + 1]), x - cta0[i] = split * blocks + query block.
+struct RagChunkSeg {
+  int64_t L, part, tiles_per_split;   // cached slots attended, first float of its partials in scratch, slot tiles per split
+  int b, T, row0, nsplit;
+};
+struct RaggedChunk {
+  Params base;                        // the call; q, out, ck, cv at row 0, the cache and sinks at slot 0
+  int n_seg, Hkv, max_pages;
+  int cta0[kMaxSeg + 1];              // first CTA of each segment (cta0[n_seg]: the grid's x extent)
+  int comb0[kMaxSeg + 1];             // first combine block of each segment (none unless it splits)
+  RagChunkSeg seg[kMaxSeg];
+};
+
+// The CTA's segment view of the call is built once in shared memory and the body reads it there: its pointers and
+// sizes stay out of the registers of a kernel that holds 240+ of them.
+template <int BITS, bool PAGED>
+__global__ void __launch_bounds__(kThreads, 1) chunk_attend_ragged_kernel(const __grid_constant__ RaggedChunk rg) {
+  __shared__ Params sp;
+  __shared__ int64_t s_qb;
+  __shared__ int s_split;
+  if (threadIdx.x == 0) {
+    const int i = find_segment(rg.cta0, rg.n_seg, (int)blockIdx.x);
+    const RagChunkSeg sg = rg.seg[i];
+    const int nqb = (sg.T + kBQ - 1) / kBQ;
+    const int local = (int)blockIdx.x - rg.cta0[i];
+    Params p = rg.base;
+    const int64_t rowq = (int64_t)sg.row0 * p.H * kHeadDim;
+    p.q += rowq;
+    p.out += rowq;
+    p.ck += (int64_t)sg.row0 * kHeadDim;
+    p.cv += (int64_t)sg.row0 * kHeadDim;
+    p.part += sg.part;
+    p.L = sg.L; p.T = sg.T; p.nsplit = sg.nsplit; p.tiles_per_split = sg.tiles_per_split;
+    const int64_t b = sg.b;
+    if (p.ns > 0) {
+      p.sink_k += b * rg.Hkv * kHeadDim * p.ns;
+      p.sink_v += b * rg.Hkv * kHeadDim * p.ns;
+    }
+    if constexpr (PAGED) {
+      p.pages += b * rg.max_pages;
+    } else {
+      const int64_t words = (int64_t)rg.Hkv * Layout<BITS>::kWords * p.Lmax, rows = p.Lmax * p.n_out;
+      p.kcache += b * words; p.vcache += b * words;
+      p.vaff += b * p.Lmax * 2;
+      if (p.kout != nullptr) { p.kout += b * rows; p.kidx += b * rows; }
+      if (p.vout != nullptr) { p.vout += b * rows; p.vidx += b * rows; }
+    }
+    sp = p;
+    s_qb = local % nqb;
+    s_split = local / nqb;
+  }
+  __syncthreads();
+  chunk_attend_body<BITS, PAGED ? kRaggedPaged : kRagged>(sp, s_qb, blockIdx.y, s_split);
+}
+
+// the lone combine of every segment that split, one block per (row, head) of those segments
+__global__ void __launch_bounds__(kHeadDim) chunk_combine_ragged_kernel(const __grid_constant__ RaggedChunk rg) {
+  const int i = find_segment(rg.comb0, rg.n_seg, (int)blockIdx.x);
+  const RagChunkSeg& sg = rg.seg[i];
+  combine_row(rg.base.part + sg.part, rg.base.out + (int64_t)sg.row0 * rg.base.H * kHeadDim,
+              (int64_t)sg.T * rg.base.H, sg.nsplit, (int)blockIdx.x - rg.comb0[i], threadIdx.x);
 }
 
 // key splits: only when the (query block, head) CTAs fill at most half the SMs; one split per slot tile at most
@@ -495,4 +611,162 @@ extern "C" int kvq_attend_chunk_gqa(int bits, int Hq, int Hkv, int64_t Lmax, int
   return attend_chunk_impl(bits, Hq, Hkv, Lmax, L, T, q, chunk_k, chunk_v, kcache, klut, k_outliers, k_outlier_idx,
                            vcache, v_cent, v_aff, v_outliers, v_outlier_idx, n_out, rope_cos_sin, rope_npos, pos_offset,
                            sink_k, sink_v, n_sink, out, scratch, stream);
+}
+
+// ---- ragged entry points ------------------------------------------------------------------------------------------
+namespace kvq {
+namespace chunk {
+
+// segments checked; segment i's partials start at the sum of the earlier segments' kvq_attend_chunk_scratch_bytes
+template <int BITS>
+int launch_ragged(RaggedChunk& rg, const int64_t* segs, cudaStream_t st, bool paged) {
+  const size_t smem = Smem<BITS>::kBytes;
+  static PerDeviceOnce attr_once[2];
+  bool& attr_done = attr_once[paged].cur();
+  if (!attr_done) {
+    cudaError_t e = paged ? cudaFuncSetAttribute(chunk_attend_ragged_kernel<BITS, true>,
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                          : cudaFuncSetAttribute(chunk_attend_ragged_kernel<BITS, false>,
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    attr_done = true;
+  }
+  int dev = 0, sms = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e != cudaSuccess) return (int)e;
+  const int H = rg.base.H;
+  int64_t ctas = 0, combs = 0, part = 0;
+  for (int i = 0; i < rg.n_seg; ++i) {
+    RagChunkSeg& sg = rg.seg[i];
+    sg.b = (int)segs[4 * i]; sg.L = segs[4 * i + 1]; sg.T = (int)segs[4 * i + 2]; sg.row0 = (int)segs[4 * i + 3];
+    sg.nsplit = sg.T > 0 ? n_splits(sg.T, H, sg.L, sms) : 1;   // the lone call's rule for (T, L)
+    const int64_t slot_tiles = (sg.L + kBK - 1) / kBK;
+    sg.tiles_per_split = sg.nsplit > 1 ? (slot_tiles + sg.nsplit - 1) / sg.nsplit : max(slot_tiles, (int64_t)1);
+    sg.part = part;
+    rg.cta0[i] = (int)ctas;
+    rg.comb0[i] = (int)combs;
+    ctas += (int64_t)(sg.T + kBQ - 1) / kBQ * sg.nsplit;
+    if (sg.nsplit > 1) combs += (int64_t)sg.T * H;
+    if (sg.T > 0) part += kvq_attend_chunk_scratch_bytes(H, sg.T, sg.L) / (int64_t)sizeof(float);
+  }
+  rg.cta0[rg.n_seg] = (int)ctas;
+  rg.comb0[rg.n_seg] = (int)combs;
+  const dim3 grid((unsigned)ctas, (unsigned)H);
+  if (paged) chunk_attend_ragged_kernel<BITS, true><<<grid, kThreads, smem, st>>>(rg);
+  else chunk_attend_ragged_kernel<BITS, false><<<grid, kThreads, smem, st>>>(rg);
+  KVQ_LAUNCH_CHECK();
+  if (combs > 0) {
+    chunk_combine_ragged_kernel<<<(unsigned)combs, kHeadDim, 0, st>>>(rg);
+    KVQ_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
+}  // namespace chunk
+}  // namespace kvq
+
+extern "C" int64_t kvq_attend_chunk_ragged_scratch_bytes(int Hq, int n_seg, const int64_t* segs) {
+  if (Hq <= 0 || n_seg < 0 || n_seg > kMaxSeg || (n_seg > 0 && segs == nullptr)) return 0;
+  int64_t total = 0;
+  for (int i = 0; i < n_seg; ++i) {
+    const int64_t L = segs[4 * i + 1], T = segs[4 * i + 2];
+    if (L < 0 || T < 0) return 0;
+    if (T > 0) total += kvq_attend_chunk_scratch_bytes(Hq, T, L);
+  }
+  return total;
+}
+
+// the ragged chunk attend over a contiguous batch (pg == nullptr) or a page pool (n_mapped: host, one per segment):
+// attend_chunk_impl's checks in its order, with the segment table's after its size checks and rope_npos checked against
+// the largest s0, then one launch (two when a segment splits)
+static int attend_chunk_ragged_impl(int bits, int B, int Hq, int Hkv, int64_t Lmax, int n_seg, const int64_t* segs,
+                                    int64_t N, const float* q, const void* chunk_k, const void* chunk_v,
+                                    const int32_t* kcache, const float* klut, const float* k_outliers,
+                                    const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent,
+                                    const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx, int n_out,
+                                    const float* rope_cos_sin, int64_t rope_npos, int pos_offset, const void* sink_k,
+                                    const void* sink_v, int n_sink, float* out, void* scratch, void* stream,
+                                    const PageRef* pg, const int32_t* n_mapped) {
+  if (bits < 2 || bits > 4) return KVQ_E_BITS;
+  if (Hq <= 0 || (Hq & 3) != 0 || Hq > 64 || Lmax <= 0) return KVQ_E_SHAPE;
+  if (B < 1 || B > kMaxSeg || n_seg < 0 || n_seg > B || N < 0) return KVQ_E_SHAPE;
+  if (Hkv <= 0 || ((Hkv & 3) != 0 && Hkv > 2) || Hq % Hkv != 0) return KVQ_E_SHAPE;
+  if (n_out < 0 || (n_out & 1) != 0 || n_out > kMaxOutDq) return KVQ_E_SHAPE;
+  if (n_sink < 0 || pos_offset < 0) return KVQ_E_SHAPE;
+  if (n_seg > 0 && (segs == nullptr || (pg != nullptr && n_mapped == nullptr))) return KVQ_E_NULL;
+  int64_t max_s0 = 0;
+  const int rc = check_segments(B, n_seg, segs, N, Lmax, pg != nullptr ? n_mapped : nullptr,
+                                pg != nullptr ? pg->max_pages : 0, pg != nullptr ? pg->P : 0, false, &max_s0);
+  if (rc) return rc;
+  if (rope_npos < (int64_t)pos_offset + max_s0) return KVQ_E_SHAPE;
+  if (N == 0) return 0;   // nothing to attend: no launch
+  if (!q || !chunk_k || !chunk_v || !out || !scratch) return KVQ_E_NULL;
+  if (!kcache || !klut || !vcache || !v_cent || !v_aff || !rope_cos_sin) return KVQ_E_NULL;
+  if ((k_outliers == nullptr) != (k_outlier_idx == nullptr) || (v_outliers == nullptr) != (v_outlier_idx == nullptr))
+    return KVQ_E_NULL;
+  if ((k_outliers || v_outliers) && n_out == 0) return KVQ_E_SHAPE;
+  if (n_sink > 0 && (!sink_k || !sink_v)) return KVQ_E_NULL;
+  if (pg != nullptr && pg->table == nullptr) return KVQ_E_NULL;
+  if ((reinterpret_cast<uintptr_t>(q) & 15) != 0 || (reinterpret_cast<uintptr_t>(chunk_k) & 15) != 0 ||
+      (reinterpret_cast<uintptr_t>(chunk_v) & 15) != 0 || (reinterpret_cast<uintptr_t>(out) & 7) != 0 ||
+      (reinterpret_cast<uintptr_t>(scratch) & 7) != 0)
+    return KVQ_E_ALIGN;
+
+  chunk::RaggedChunk rg{};        // ~12 KB, passed to the kernels by value
+  chunk::Params& p = rg.base;
+  p.q = q;
+  p.ck = static_cast<const __half*>(chunk_k);
+  p.cv = static_cast<const __half*>(chunk_v);
+  p.kcache = kcache; p.klut = klut; p.kout = k_outliers; p.kidx = k_outlier_idx;
+  p.vcache = vcache; p.vcent = v_cent; p.vaff = v_aff; p.vout = v_outliers; p.vidx = v_outlier_idx;
+  p.rope = reinterpret_cast<const float2*>(rope_cos_sin); p.npos = rope_npos; p.pos0 = pos_offset;
+  p.sink_k = static_cast<const __half*>(sink_k); p.sink_v = static_cast<const __half*>(sink_v);
+  p.ns = n_sink;
+  p.out = out;
+  p.part = static_cast<float*>(scratch);
+  p.H = Hq; p.grp = Hq / Hkv; p.n_out = n_out; p.Lmax = pg != nullptr ? pg->P : Lmax;
+  p.cstride = N;
+  p.pages = pg != nullptr ? pg->table : nullptr; p.P = pg != nullptr ? pg->P : 0;
+  rg.n_seg = n_seg; rg.Hkv = Hkv; rg.max_pages = pg != nullptr ? pg->max_pages : 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  switch (bits) {
+    case 4: return chunk::launch_ragged<4>(rg, segs, st, pg != nullptr);
+    case 3: return chunk::launch_ragged<3>(rg, segs, st, pg != nullptr);
+    default: return chunk::launch_ragged<2>(rg, segs, st, pg != nullptr);
+  }
+}
+
+extern "C" int kvq_attend_chunk_ragged(int bits, int B, int Hq, int Hkv, int64_t Lmax, int n_seg, const int64_t* segs,
+                                       int64_t N, const float* q, const void* chunk_k, const void* chunk_v,
+                                       const int32_t* kcache, const float* klut, const float* k_outliers,
+                                       const int32_t* k_outlier_idx, const int32_t* vcache, const float* v_cent,
+                                       const float* v_aff, const float* v_outliers, const int32_t* v_outlier_idx,
+                                       int n_out, const float* rope_cos_sin, int64_t rope_npos, int pos_offset,
+                                       const void* sink_k, const void* sink_v, int n_sink, float* out, void* scratch,
+                                       void* stream) {
+  return attend_chunk_ragged_impl(bits, B, Hq, Hkv, Lmax, n_seg, segs, N, q, chunk_k, chunk_v, kcache, klut, k_outliers,
+                                  k_outlier_idx, vcache, v_cent, v_aff, v_outliers, v_outlier_idx, n_out, rope_cos_sin,
+                                  rope_npos, pos_offset, sink_k, sink_v, n_sink, out, scratch, stream, nullptr, nullptr);
+}
+
+extern "C" int kvq_attend_chunk_ragged_paged(int bits, int B, int Hq, int Hkv, int n_pool, int n_seg,
+                                             const int64_t* segs, int64_t N, const float* q, const void* chunk_k,
+                                             const void* chunk_v, const int32_t* kcache, const float* klut,
+                                             const float* k_outliers, const int32_t* k_outlier_idx,
+                                             const int32_t* vcache, const float* v_cent, const float* v_aff,
+                                             const float* v_outliers, const int32_t* v_outlier_idx, int n_out,
+                                             const float* rope_cos_sin, int64_t rope_npos, int pos_offset,
+                                             const void* sink_k, const void* sink_v, int n_sink, float* out,
+                                             void* scratch, void* stream, const int32_t* page_table, int max_pages,
+                                             const int32_t* n_mapped, int P) {
+  if (bits < 2 || bits > 4) return KVQ_E_BITS;
+  if (Hkv <= 0 || ((Hkv & 3) != 0 && Hkv > 2)) return KVQ_E_SHAPE;
+  const int rc = check_pages(n_pool, max_pages, P, (int64_t)Hkv * kHeadDim * bits / 32);
+  if (rc) return rc;
+  const PageRef pg{page_table, nullptr, max_pages, P, n_pool};
+  return attend_chunk_ragged_impl(bits, B, Hq, Hkv, (int64_t)max_pages * P, n_seg, segs, N, q, chunk_k, chunk_v, kcache,
+                                  klut, k_outliers, k_outlier_idx, vcache, v_cent, v_aff, v_outliers, v_outlier_idx,
+                                  n_out, rope_cos_sin, rope_npos, pos_offset, sink_k, sink_v, n_sink, out, scratch,
+                                  stream, &pg, n_mapped);
 }

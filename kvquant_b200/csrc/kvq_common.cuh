@@ -218,6 +218,30 @@ __device__ __forceinline__ int64_t page_row(const PageRef& pg, int s) {
   return (int64_t)pc.page * pg.P + pc.col;
 }
 
+// Ragged calls (kvq_append_kv_fused_chunk_ragged*, kvq_attend_chunk_ragged*; DESIGN.md section 4.15): a host segment
+// table segs int64 [n_seg][4] of (slot b, first slot s0, T, first row) packs several slots' chunks into one launch.
+// The table travels to the kernels by value (as a __grid_constant__ parameter), so n_seg is bounded by the batch.
+constexpr int kMaxSeg = 256;
+
+// host: the segment checks of the ragged entry points (kvq_page.cu), in order: slots in [0, B) and distinct, s0 >= 0,
+// T >= 0, rows packed in segment order (row0 = the earlier segments' T), s0 + T <= Lmax (the per-slot cap), and when
+// n_mapped is given 0 <= n_mapped[i] <= max_pages with the slots the call touches mapped: s0 + T for a call that writes
+// them (the append), s0 for one that reads the first s0 (the attend); N = the sum of T and N < 2^31 -> KVQ_E_SHAPE.
+// *max_s0 (optional) receives the largest s0.
+int check_segments(int B, int n_seg, const int64_t* segs, int64_t N, int64_t Lmax, const int32_t* n_mapped,
+                   int max_pages, int P, bool writes, int64_t* max_s0);
+
+// device: the last i < n with first[i] <= x (first[] non-decreasing, first[0] == 0), i.e. the segment owning block x of
+// a ragged grid; a segment of no blocks shares its start with the next one and is never returned
+__device__ __forceinline__ int find_segment(const int* first, int n, int x) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (first[mid] <= x) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
 // host: build a 2D tensor map over the packed cache viewed as uint32 [rows = H*W, cols = Lmax]  (kvq_capi.cu)
 int make_cache_tensor_map(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                           uint32_t box_cols, uint32_t box_rows, int swizzle_bytes);

@@ -18,6 +18,28 @@ int check_pages(int n_pool, int max_pages, int P, int64_t rows) {
   return 0;
 }
 
+int check_segments(int B, int n_seg, const int64_t* segs, int64_t N, int64_t Lmax, const int32_t* n_mapped,
+                   int max_pages, int P, bool writes, int64_t* max_s0) {
+  bool seen[kMaxSeg] = {};
+  int64_t row = 0, top = 0;
+  for (int i = 0; i < n_seg; ++i) {
+    const int64_t b = segs[4 * i], s0 = segs[4 * i + 1], T = segs[4 * i + 2], row0 = segs[4 * i + 3];
+    if (b < 0 || b >= B || seen[b]) return KVQ_E_SHAPE;
+    seen[b] = true;
+    if (s0 < 0 || T < 0 || row0 != row) return KVQ_E_SHAPE;
+    if (s0 > Lmax || T > Lmax - s0) return KVQ_E_SHAPE;
+    if (n_mapped != nullptr) {   // the slots read (s0) or written (s0 + T) must be mapped
+      if (n_mapped[i] < 0 || n_mapped[i] > max_pages) return KVQ_E_SHAPE;
+      if ((writes ? s0 + T : s0) > (int64_t)n_mapped[i] * P) return KVQ_E_SHAPE;
+    }
+    row += T;
+    top = std::max(top, s0);
+  }
+  if (row != N || N >= ((int64_t)1 << 31)) return KVQ_E_SHAPE;
+  if (max_s0 != nullptr) *max_s0 = top;
+  return 0;
+}
+
 // one side of a copy: the eight tensors as 32-bit words (kcache, vcache, k values, k indices, v values, v indices,
 // vlut, (sf, off)); pages == nullptr: a contiguous cache of Lmax slots
 struct CopySide {

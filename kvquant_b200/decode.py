@@ -26,7 +26,7 @@ from dataclasses import dataclass
 
 import torch
 
-from .cache import RopeLenState, BatchedLayerCache, LayerCache, PagedLayerCache, PageTable, HEAD_DIM
+from .cache import RopeLenState, BatchedLayerCache, LayerCache, PagedLayerCache, PageTable, HEAD_DIM, _resolve
 from .rope import LengthDependentRotary, RotarySpec
 
 
@@ -370,19 +370,31 @@ class DecoderStage:
             h = x[s0:s0 + chunk]
             n = h.shape[0]
             for ly, c in zip(self.layers, caches):
-                qkv = rmsnorm(h, ly.n1, cfg.rms_eps) @ ly.wqkv.t()
-                q, k, v = qkv.float().split((hid, cfg.kv_hidden, cfg.kv_hidden), dim=-1)
+                q, k, v = self._prefill_qkv(ly, h)
                 pos = c.n_sink + c.pos_base + c.len + torch.arange(n, device=self.device)
                 q = self._rope_rows(q.reshape(n, H, HEAD_DIM), pos).contiguous()
-                k, v = k.contiguous(), v.contiguous()
                 o = c.attend_chunk(q, k, v, rope_theta=cfg.rope_theta, rope=self.rotary)
                 c.append_chunk(k, v)
-                h = h + o.half().view(n, hid) @ ly.wo.t()
-                gu = rmsnorm(h, ly.n2, cfg.rms_eps) @ ly.wgu.t()
-                g, u = gu.split(cfg.intermediate, dim=-1)
-                h = h + (torch.nn.functional.silu(g) * u) @ ly.wdown.t()
+                h = self._prefill_out(ly, h, o)
             outs.append(h)
         return torch.cat(outs) if outs else x.clone()
+
+    def _prefill_qkv(self, ly, h):
+        """RMSNorm + the QKV projection of prompt rows h fp16 [n, hidden] (one fp16 matmul): q f32 [n, hidden] and the
+        contiguous pre-RoPE k, v f32 [n, kv_hidden].  Shared by prefill and BatchedDecoderStage.prefill_seqs."""
+        cfg = self.cfg
+        qkv = rmsnorm(h, ly.n1, cfg.rms_eps) @ ly.wqkv.t()
+        q, k, v = qkv.float().split((cfg.hidden, cfg.kv_hidden, cfg.kv_hidden), dim=-1)
+        return q, k.contiguous(), v.contiguous()
+
+    def _prefill_out(self, ly, h, o):
+        """o_proj of the attention output o f32 [n, q_heads, 128] + residual, then the MLP + residual (the math of
+        forward_torch): h fp16 [n, hidden] after the layer.  Shared by prefill and BatchedDecoderStage.prefill_seqs."""
+        cfg = self.cfg
+        h = h + o.half().view(h.shape[0], cfg.hidden) @ ly.wo.t()
+        gu = rmsnorm(h, ly.n2, cfg.rms_eps) @ ly.wgu.t()
+        g, u = gu.split(cfg.intermediate, dim=-1)
+        return h + (torch.nn.functional.silu(g) * u) @ ly.wdown.t()
 
     def _rope_rows(self, q, pos):
         """_rope_q of every row: q f32 [n, H, 128] rotated at positions pos [n]."""
@@ -607,6 +619,81 @@ class BatchedDecoderStage:
         y = self.stage.prefill(x, chunk, caches=[bc.slot(b) for bc in self.caches])
         self.caches[0].commit(b)            # (one shared page table and length tensor)
         return y
+
+    def prefill_seqs(self, prompts, chunk=2048, max_tokens=8192):
+        """prefill_seq of several prompts at once (DESIGN.md section 4.15): prompts {slot: fp16 [T_b, hidden]} ->
+        {slot: fp16 [T_b, hidden]}, every slot committed.  Each prompt continues its slot at the slot's host length --
+        an empty slot, a follow-up turn after graph replays, a fork_seq destination -- and is cut into chunks exactly
+        as prefill_seq(b, x, chunk) cuts it.  A round packs the next chunk of as many prompts as fit in max_tokens rows
+        (in the mapping's order); per layer and round one RMSNorm + QKV matmul over the packed rows, the per-row query
+        rotation, one attend_chunks, one append_chunks, then one o_proj + MLP (DecoderStage._prefill_qkv / _prefill_out).
+        So every layer reads its weights once per round instead of once per prompt and chunk.
+
+        The chunks attend through the fused ragged chunk attend, which reads the cache directly; prefill_seq attends
+        through attend_chunk (SDPA over a dequantised copy), so the two agree to fp16 rounding, not bit for bit.  A
+        prompt past the cap (IndexError), an exhausted pool or a write into a shared page (RuntimeError) raises before
+        anything is written or reserved for any slot.  Other slots are untouched and no recapture is needed.
+        Length-dependent rotary and the legacy per-token-LUT V form raise NotImplementedError: use prefill_seq."""
+        stage, cfg = self.stage, self.cfg
+        if isinstance(stage.rotary, LengthDependentRotary):
+            raise NotImplementedError("prefill_seqs with length-dependent rotary frequencies needs a frequency table per "
+                                      "slot; prefill such prompts one at a time with prefill_seq")
+        if not self.caches[0]._tmpl.use_native_v:
+            raise NotImplementedError("prefill_seqs reads the native V form; use prefill_seq for the per-token-LUT form")
+        chunk, max_tokens = int(chunk), int(max_tokens)
+        if chunk < 1 or chunk > max_tokens:
+            raise ValueError("need 1 <= chunk <= max_tokens, got chunk=%d, max_tokens=%d" % (chunk, max_tokens))
+        H, hid = cfg.n_heads, cfg.hidden
+        items = []
+        for b, x in prompts.items():
+            b = int(b)
+            if not 0 <= b < self.B:
+                raise IndexError("slot %d out of range [0, %d)" % (b, self.B))
+            if x.dtype != torch.float16 or x.dim() != 2 or x.shape[1] != hid:
+                raise ValueError("prompt of slot %d must be fp16 [T, %d], got %s %s" % (b, hid, x.dtype, tuple(x.shape)))
+            if x.device != self.device:
+                raise ValueError("prompt of slot %d is on %s, the stage lives on %s" % (b, x.device, self.device))
+            items.append((b, x))
+        if len({b for b, _ in items}) != len(items):
+            raise ValueError("prompts must name distinct slots")
+        bc0 = self.caches[0]
+        start = {b: bc0._host_len(b) for b, _ in items}
+        for b, x in items:
+            if start[b] + x.shape[0] > bc0.Lmax:
+                raise IndexError("a prompt of %d tokens does not fit slot %d: %d of %d slots used"
+                                 % (x.shape[0], b, start[b], bc0.Lmax))
+        if self.paged:    # every page of every prompt, checked together and then mapped, before any layer runs
+            bc0._map_chunks([b for b, _ in items], [start[b] for b, _ in items], [x.shape[0] for _, x in items])
+        todo = {b: list(range(0, x.shape[0], chunk)) for b, x in items}
+        outs = {b: [] for b, _ in items}
+        xs = dict(items)
+        while any(todo.values()):
+            rnd, rows = [], 0
+            for b, _ in items:              # the next chunk of every prompt that still fits in this round
+                if todo[b]:
+                    n = min(chunk, xs[b].shape[0] - todo[b][0])
+                    if rows + n <= max_tokens:
+                        rnd.append((b, todo[b].pop(0), n))
+                        rows += n
+            slots, counts = [b for b, _, _ in rnd], [n for _, _, n in rnd]
+            starts = [bc0._host_len(b) for b in slots]
+            h = torch.cat([xs[b][s0:s0 + n] for b, s0, n in rnd])
+            pos = torch.cat([bc0.n_sink + s + torch.arange(n, device=self.device) for s, n in zip(starts, counts)])
+            rope = _resolve(stage.rotary, cfg.rope_theta)
+            for ly, bc in zip(stage.layers, self.caches):
+                q, k, v = stage._prefill_qkv(ly, h)
+                q = stage._rope_rows(q.reshape(rows, H, HEAD_DIM), pos).contiguous()
+                o = bc._attend_chunks_at(slots, starts, q, k, v, counts, rope)
+                bc._append_chunks_at(slots, starts, k, v, counts)
+                h = stage._prefill_out(ly, h, o)
+            for b, s, n in zip(slots, starts, counts):
+                for bc in (self.caches if not self.paged else self.caches[:1]):   # (paged: one shared table)
+                    bc._set_host_len(b, s + n)
+            for (b, _, _), y in zip(rnd, h.split(counts)):
+                outs[b].append(y)
+        for b, x in items:
+            self.caches[0].commit(b)        # (one shared length tensor)
+        return {b: torch.cat(outs[b]) if outs[b] else x.clone() for b, x in items}
 
     def fork_seq(self, src, dst):
         """Paged: slot dst continues from slot src's current tokens, sharing its full pages in every layer and
